@@ -5,12 +5,14 @@
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
+#include <array>
 #include <cstring>
 #include <map>
 #include <memory>
 #include <mutex>
 #include <vector>
 #include "../../include/hbls.h"
+#include "coalesce.hpp"
 #include "kernels.cuh"
 
 using namespace hb;
@@ -56,6 +58,7 @@ struct Ctx {
     g2a* hm_slots = nullptr; uint8_t* hm_ok = nullptr; HmEntry hm[HM_N];
     uint64_t hm_clock = 0, hm_hits = 0, hm_misses = 0;
     long long hm_cache = 1;                                 // hbls_set_param("hm_cache", 0) turns it off (cold-path measurements)
+    hbls_coalesce::Combiner part1;                          // concurrent herumi-API calls (include/hbls.h part 1) -> shared turns
 };
 Ctx g;
 
@@ -107,20 +110,22 @@ inline unsigned blocks_for(size_t n, unsigned tpb) { return (unsigned)((n + tpb 
 // whatever stream the call runs on; `filled` orders readers after the fill, `read_done` orders a later overwrite after the readers.
 void hm_key(uint8_t key[48], const void* msg, size_t len) { memset(key, 0, 48); if (len) memcpy(key, msg, len > 48 ? 48 : len); }
 bool hm_enabled() { return g.hm_cache != 0 && g.hm_slots != nullptr; }
+// the cache slot holding key, or -1
+int hm_find(const uint8_t key[48]) {
+    for (int i = 0; i < Ctx::HM_N; i++) if (g.hm[i].used && memcmp(g.hm[i].key, key, 48) == 0) return i;
+    return -1;
+}
 // hit: stream st copies the cached point into dst / dst_ok and true is returned
 bool hm_fetch(const uint8_t key[48], g2a* dst, uint8_t* dst_ok, cudaStream_t st) {
-    for (int i = 0; i < Ctx::HM_N; i++) {
-        Ctx::HmEntry& e = g.hm[i];
-        if (!e.used || memcmp(e.key, key, 48) != 0) continue;
-        cudaStreamWaitEvent(st, e.filled, 0);
-        cudaMemcpyAsync(dst, g.hm_slots + i, sizeof(g2a), cudaMemcpyDeviceToDevice, st);
-        cudaMemcpyAsync(dst_ok, g.hm_ok + i, 1, cudaMemcpyDeviceToDevice, st);
-        cudaEventRecord(e.read_done, st); e.has_reader = true;
-        e.stamp = ++g.hm_clock; g.hm_hits++;
-        return true;
-    }
-    g.hm_misses++;
-    return false;
+    const int i = hm_find(key);
+    if (i < 0) { g.hm_misses++; return false; }
+    Ctx::HmEntry& e = g.hm[i];
+    cudaStreamWaitEvent(st, e.filled, 0);
+    cudaMemcpyAsync(dst, g.hm_slots + i, sizeof(g2a), cudaMemcpyDeviceToDevice, st);
+    cudaMemcpyAsync(dst_ok, g.hm_ok + i, 1, cudaMemcpyDeviceToDevice, st);
+    cudaEventRecord(e.read_done, st); e.has_reader = true;
+    e.stamp = ++g.hm_clock; g.hm_hits++;
+    return true;
 }
 // after stream st has produced H(key) in src / src_ok: keep a copy in the least recently used slot
 void hm_store(const uint8_t key[48], const g2a* src, const uint8_t* src_ok, cudaStream_t st) {
@@ -301,7 +306,7 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
             else LAUNCH(k_hash_to_g2, 1, TPB, sh, (size_t)1, d_msgs, msg_len, v.hm, v.ok_hm);
             if (use_cache) hm_store(key, v.hm, v.ok_hm, sh);
         }
-        if (B > 1) LAUNCH(k_broadcast_hm, blocks_for(B, 256), 256, sh, B, v.hm, v.ok_hm);
+        if (B > 1) LAUNCH(k_broadcast_hm, blocks_for(B, 256), 256, sh, B, (const uint32_t*)nullptr, (const g2a*)v.hm, (const uint8_t*)v.ok_hm, v.hm, v.ok_hm);
     } else if (pairs)
         launch_hash_small(sh, B, d_msgs, msg_len, v.hm, v.ok_hm);
     else if (g.hash_split && HB_BATCH_INV) {
@@ -444,25 +449,6 @@ void launch_exact_two_phase(size_t n, const g2a* sig, const g1a* pkneg, const g2
     LAUNCH(k_exact_publish, blocks_for(n, 256), 256, s, n, (const uint32_t*)nullptr, (const uint8_t*)verdict, d_results);
 }
 
-int single_op(int op, const void* a, size_t an, const void* b, size_t bn, void* out, size_t on, int* rc_out, uint32_t len = 0) {
-    if (int e = ensure_init()) return e;
-    std::lock_guard<std::mutex> lk(g.mu);
-    Scratch* sc; if (int e = reserve(g.stream, an + bn + on + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* da = ar.take<uint8_t>(an ? an : 1); uint8_t* db = ar.take<uint8_t>(bn ? bn : 1);
-    uint8_t* dout = ar.take<uint8_t>(on ? on : 1); int* drc = ar.take<int>(1);
-    if (an) CK(cudaMemcpyAsync(da, a, an, cudaMemcpyHostToDevice, g.stream));
-    if (bn) CK(cudaMemcpyAsync(db, b, bn, cudaMemcpyHostToDevice, g.stream));
-    LAUNCH(k_single, 1, 32, g.stream, op, da, db, dout, drc, len);
-    int rc = 0;
-    CK(cudaMemcpyAsync(&rc, drc, sizeof(int), cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    if (on && rc >= 0 && !((op == OP_G1_DES || op == OP_G2_DES) && rc == 0) && !(op == OP_MAP_SER && rc != 0))
-        CK(cudaMemcpy(out, dout, on, cudaMemcpyDeviceToHost));
-    *rc_out = rc;
-    return 0;
-}
-
 // sk (little-endian u64 x 4, < r < Z^4) -> its four base-Z digits, Z = |z| = 0xd201000000010000 (plain long division on the host)
 bool sk_digits_base_z(const uint64_t sk[4], uint64_t dig[4]) {
     const uint64_t Z = 0xd201000000010000ull;
@@ -481,6 +467,160 @@ const uint64_t R_ORDER[4] = {0xffffffff00000001ull, 0x53bda402fffe5bfeull, 0x333
 bool scalar_lt_r(const uint64_t k[4]) {
     for (int i = 3; i >= 0; i--) { if (k[i] < R_ORDER[i]) return true; if (k[i] > R_ORDER[i]) return false; }
     return false;
+}
+
+// ------------------------------------------------------------------ herumi-API calls (part 1 of include/hbls.h), n requests at a
+// time.  Concurrent calls from different threads are combined into turns (coalesce.hpp); a turn stages the inputs of all its requests
+// with one copy, runs each kernel once over the requests that need it and copies the results back once.  A lone call is a turn of
+// one and launches the kernels a call has always launched.
+enum { RQ_VERIFY, RQ_SIGN, RQ_PUBKEY, RQ_SINGLE };
+constexpr size_t PART1_CAP = 1024;       // sign / GetPublicKey / single-element requests per turn (verify: coop_max, the warp-per-round limit)
+struct Part1Req : hbls_coalesce::Request {
+    const void* a = nullptr; const void* b = nullptr;   // VERIFY: signature, public key; SIGN / PUBKEY: secret key; SINGLE: operands
+    size_t an = 0, bn = 0;                              // SINGLE: operand bytes
+    const void* msg = nullptr; size_t len = 0;          // VERIFY / SIGN: the hash (first 48 bytes); SINGLE: the message length
+    void* out = nullptr; size_t on = 0;                 // SIGN / PUBKEY: the result struct; SINGLE: the result bytes
+    int op = 0;                                         // SINGLE: OP_*
+    int err = 0;                                        // HBLS_ERR_CUDA when the turn's device work failed (nothing written)
+    int rc = 0;                                         // VERIFY: 1 / 0; SIGN: 0 / -1; SINGLE: the op's return code
+};
+static_assert(sizeof(g1) == sizeof(blsPublicKey) && sizeof(g2) == sizeof(blsSignature), "herumi struct layout");
+// byte layout of one staging copy: 256-byte aligned sections
+struct Layout {
+    size_t size = 0;
+    size_t put(size_t bytes) { const size_t off = (size + 255) & ~(size_t)255; size = off + (bytes ? bytes : 1); return off; }
+};
+
+// One turn: the requests rq[0..n) under g.mu.  d_apk / sig96 (hbls_mask_verify: one verify request): the key is already on the
+// device and the signature is serialized (decoded and subgroup-checked here).  Fills in each request's results and returns 0, or
+// HBLS_ERR_CUDA with no result written.
+int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const uint8_t* sig96 = nullptr) {
+    cudaStream_t s = g.stream;
+    std::vector<Part1Req*> ver, sgn, pub, one;
+    for (size_t i = 0; i < n; i++) (rq[i]->kind == RQ_VERIFY ? ver : rq[i]->kind == RQ_SIGN ? sgn : rq[i]->kind == RQ_PUBKEY ? pub : one).push_back(rq[i]);
+    // signing keys in base |z| first (ladder over psi), hand-filled keys >= Z^4 after them (plain ladder)
+    std::vector<uint64_t> dig; size_t ngls = 0;
+    {
+        std::vector<Part1Req*> rest;
+        for (Part1Req* r : sgn) {
+            uint64_t d[4];
+            if (sk_digits_base_z(static_cast<const blsSecretKey*>(r->a)->d, d)) { sgn[ngls++] = r; dig.insert(dig.end(), d, d + 4); }
+            else rest.push_back(r);
+        }
+        std::copy(rest.begin(), rest.end(), sgn.begin() + ngls);
+    }
+    const size_t nv = ver.size(), ns = sgn.size(), np = pub.size(), n1 = one.size(), nh = nv + ns;
+    // H(m): one table entry per distinct message of the verify and sign requests (the key hm_key builds); entries the cache holds at
+    // the back, the misses at the front (contiguous: one hash launch), idx[i] = entry of request i (verify requests, then sign)
+    std::vector<std::array<uint8_t, 48>> keys; std::vector<uint32_t> idx(nh);
+    {
+        std::map<std::array<uint8_t, 48>, uint32_t> seen;
+        for (size_t i = 0; i < nh; i++) {
+            const Part1Req* r = i < nv ? ver[i] : sgn[i - nv];
+            std::array<uint8_t, 48> k; hm_key(k.data(), r->msg, r->len);
+            auto it = seen.emplace(k, (uint32_t)keys.size());
+            if (it.second) keys.push_back(k);
+            idx[i] = it.first->second;
+        }
+    }
+    const size_t nk = keys.size();
+    std::vector<uint32_t> pos(nk); std::vector<bool> cached(nk, false); size_t nmiss = 0;
+    for (size_t d = 0; d < nk; d++) cached[d] = hm_enabled() && hm_find(keys[d].data()) >= 0;
+    for (size_t d = 0, hit = 0; d < nk; d++) pos[d] = cached[d] ? (uint32_t)(nk - 1 - hit++) : (uint32_t)nmiss++;
+    bool gather = nk != nh;
+    for (size_t i = 0; i < nh; i++) { idx[i] = pos[idx[i]]; gather |= idx[i] != i; }
+    // staging (host -> device, one copy) and results (device -> host, one copy)
+    Layout in, out;
+    const size_t i_apk = d_apk ? 0 : in.put(nv * sizeof(g1)), i_sig = in.put(sig96 ? 96 : nv * sizeof(g2)), i_keys = in.put(nmiss * 48);
+    const size_t i_idx = gather ? in.put(nh * 4) : 0, i_dig = in.put(dig.size() * 8), i_sk = in.put((ns - ngls) * 32), i_pub = in.put(np * 32);
+    std::vector<size_t> i_a(n1), i_b(n1), o_out(n1);
+    for (size_t j = 0; j < n1; j++) { i_a[j] = in.put(one[j]->an); i_b[j] = in.put(one[j]->bn); o_out[j] = out.put(one[j]->on); }
+    const size_t i_desc = n1 > 1 ? in.put(n1 * sizeof(single_desc)) : 0;
+    const size_t o_res = out.put(nv), o_sig = out.put(ns * sizeof(g2)), o_sok = out.put(ns), o_pub = out.put(np * sizeof(g1)), o_rc = out.put(n1 * sizeof(int));
+    Scratch* sc;
+    if (int e = reserve(s, in.size + out.size + nv * (sizeof(g1a) + sizeof(g2a) + 1) + (nk + nh) * (sizeof(g2a) + 1) + 16 * 256, &sc)) return e;
+    Arena ar{sc->base, 0, sc->cap};
+    uint8_t* din = ar.take<uint8_t>(in.size); uint8_t* dout = ar.take<uint8_t>(out.size);
+    g1a* pkneg = ar.take<g1a>(nv); g2a* vsig = ar.take<g2a>(nv); uint8_t* ok_sig = ar.take<uint8_t>(nv);
+    g2a* hm = ar.take<g2a>(nh); uint8_t* ok_hm = ar.take<uint8_t>(nh);
+    g2a* th = gather ? ar.take<g2a>(nk) : hm; uint8_t* tok = gather ? ar.take<uint8_t>(nk) : ok_hm;      // the H(m) table
+    std::vector<uint8_t> hin(in.size), hout(out.size);
+    for (size_t i = 0; i < nv && !d_apk; i++) memcpy(&hin[i_apk + i * sizeof(g1)], ver[i]->b, sizeof(g1));
+    if (sig96) memcpy(&hin[i_sig], sig96, 96);
+    else for (size_t i = 0; i < nv; i++) memcpy(&hin[i_sig + i * sizeof(g2)], ver[i]->a, sizeof(g2));
+    for (size_t d = 0; d < nk; d++) if (!cached[d]) memcpy(&hin[i_keys + 48 * pos[d]], keys[d].data(), 48);
+    if (gather) memcpy(&hin[i_idx], idx.data(), nh * 4);
+    if (!dig.empty()) memcpy(&hin[i_dig], dig.data(), dig.size() * 8);
+    for (size_t i = ngls; i < ns; i++) memcpy(&hin[i_sk + 32 * (i - ngls)], static_cast<const blsSecretKey*>(sgn[i]->a)->d, 32);
+    for (size_t i = 0; i < np; i++) memcpy(&hin[i_pub + 32 * i], static_cast<const blsSecretKey*>(pub[i]->a)->d, 32);
+    std::vector<single_desc> desc(n1);
+    for (size_t j = 0; j < n1; j++) {
+        if (one[j]->an) memcpy(&hin[i_a[j]], one[j]->a, one[j]->an);
+        if (one[j]->bn) memcpy(&hin[i_b[j]], one[j]->b, one[j]->bn);
+        desc[j] = single_desc{din + i_a[j], din + i_b[j], dout + o_out[j], one[j]->op, (uint32_t)one[j]->len};
+    }
+    if (n1 > 1) memcpy(&hin[i_desc], desc.data(), n1 * sizeof(single_desc));
+    CK(cudaMemcpyAsync(din, hin.data(), in.size, cudaMemcpyHostToDevice, s));
+    int* drc = reinterpret_cast<int*>(dout + o_rc);
+    if (n1) LAUNCH(k_single, blocks_for(n1, 32), 32, s, n1, n1 > 1 ? (const single_desc*)(din + i_desc) : (const single_desc*)nullptr, desc[0], drc);
+    if (np) LAUNCH(k_g1_mul_gen, blocks_for(np, 32), 32, s, np, (const uint8_t*)(din + i_pub), reinterpret_cast<g1*>(dout + o_pub));
+    const uint8_t* vok_sig = nullptr;
+    if (nv) {
+        LAUNCH(k_g1_normalize_lat, blocks_for(nv, 32), 32, s, nv, d_apk ? d_apk : reinterpret_cast<const g1*>(din + i_apk), pkneg, 1);
+        if (sig96) { LAUNCH(k_g2_decode_pair, 1, 32, s, (size_t)1, (const uint8_t*)(din + i_sig), vsig, ok_sig, 1); vok_sig = ok_sig; }
+        else LAUNCH(k_g2_normalize, blocks_for(nv, 32), 32, s, nv, reinterpret_cast<const g2*>(din + i_sig), vsig);
+    }
+    // H(m): cached entries (this node signed, verified or prefetched the message before), then one launch over the misses
+    for (size_t d = 0; d < nk; d++) if (cached[d]) hm_fetch(keys[d].data(), th + pos[d], tok + pos[d], s);
+    if (hm_enabled()) g.hm_misses += nmiss;
+    if (nmiss) {
+        launch_hash_small(s, nmiss, din + i_keys, 48, th, tok);
+        if (hm_enabled()) for (size_t d = 0; d < nk; d++) if (!cached[d]) hm_store(keys[d].data(), th + pos[d], tok + pos[d], s);
+    }
+    if (gather) LAUNCH(k_broadcast_hm, blocks_for(nh, 256), 256, s, nh, (const uint32_t*)(din + i_idx), (const g2a*)th, (const uint8_t*)tok, hm, ok_hm);
+    if (nv) {
+        uint8_t* dres = dout + o_res;
+        const size_t coop_cap = (size_t)g.sm_count * (size_t)(g.coop_wpsm > 0 ? g.coop_wpsm : 1);
+        if (g.coop_max >= 1) LAUNCH(k_pairing_coop, (unsigned)(nv < coop_cap ? nv : coop_cap), 32, s, nv, vsig, pkneg, hm, (const uint8_t*)ok_hm, vok_sig, (const uint8_t*)nullptr, dres);
+        else LAUNCH(k_pairing_verify_split, blocks_for(2 * nv, 64), 64, s, nv, vsig, pkneg, hm, (const uint8_t*)ok_hm, vok_sig, (const uint8_t*)nullptr, dres, (const int*)nullptr);
+        LAUNCH(k_pairing_fixup, blocks_for(nv, 32), 32, s, nv, vsig, pkneg, hm, (const uint8_t*)ok_hm, vok_sig, (const uint8_t*)nullptr, dres, (const int*)nullptr);
+    }
+    g2* dsig_out = reinterpret_cast<g2*>(dout + o_sig); uint8_t* dsok = dout + o_sok;
+    if (ngls) LAUNCH(k_sign_hm_gls_pair, blocks_for(2 * ngls, 32), 32, s, ngls, (const uint64_t*)(din + i_dig), hm + nv, (const uint8_t*)ok_hm + nv, (size_t)1, dsig_out, dsok);
+    if (ns > ngls) LAUNCH(k_sign_hm_pair, blocks_for(2 * (ns - ngls), 32), 32, s, ns - ngls, (const uint8_t*)(din + i_sk), hm + nv + ngls, (const uint8_t*)ok_hm + nv + ngls,
+                          (size_t)1, dsig_out + ngls, dsok + ngls);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(hout.data(), dout, out.size, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (size_t i = 0; i < nv; i++) ver[i]->rc = hout[o_res + i] ? 1 : 0;
+    for (size_t i = 0; i < ns; i++) { memcpy(sgn[i]->out, &hout[o_sig + i * sizeof(g2)], sizeof(g2)); sgn[i]->rc = hout[o_sok + i] ? 0 : -1; }
+    for (size_t i = 0; i < np; i++) memcpy(pub[i]->out, &hout[o_pub + i * sizeof(g1)], sizeof(g1));
+    for (size_t j = 0; j < n1; j++) {
+        Part1Req& r = *one[j]; int rc; memcpy(&rc, &hout[o_rc + j * sizeof(int)], sizeof(int));
+        if (r.on && rc >= 0 && !((r.op == OP_G1_DES || r.op == OP_G2_DES) && rc == 0) && !(r.op == OP_MAP_SER && rc != 0)) memcpy(r.out, &hout[o_out[j]], r.on);
+        r.rc = rc;
+    }
+    return 0;
+}
+
+// runs r in a turn of the combiner (from any thread; the caller must not hold g.mu)
+void part1_submit(Part1Req& r) {
+    g.part1.submit(r, g.mu,
+        [](int kind) { return kind == RQ_VERIFY ? (size_t)(g.coop_max > 0 ? g.coop_max : 1) : PART1_CAP; },
+        [](hbls_coalesce::Request** rq, size_t n) {
+            std::vector<Part1Req*> turn(n);
+            for (size_t i = 0; i < n; i++) turn[i] = static_cast<Part1Req*>(rq[i]);
+            const int e = part1_locked(turn.data(), n);
+            for (Part1Req* r : turn) r->err = e;
+        });
+}
+int single_op(int op, const void* a, size_t an, const void* b, size_t bn, void* out, size_t on, int* rc_out, uint32_t len = 0) {
+    if (int e = ensure_init()) return e;
+    Part1Req r; r.kind = RQ_SINGLE; r.op = op; r.a = a; r.an = an; r.b = b; r.bn = bn; r.out = out; r.on = on; r.len = len;
+    part1_submit(r);
+    if (r.err) return r.err;
+    *rc_out = r.rc;
+    return 0;
 }
 
 // SHA-256 (host; GetAddress = first 20 bytes of SHA-256 of the serialized key)
@@ -617,6 +757,31 @@ int agg_verify_device_locked(const hbls_committee* c, size_t B, const uint8_t* d
         LAUNCH(k_mask_aggregate, blocks_for(B * 32, 128), 128, s, B, c->n, c->table, d_bitmaps, blen, v.apk);
     launch_verify_tail(B, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, same_msg, h_msg);
     if (v_out) *v_out = v;
+    return 0;
+}
+// Mask.SetMask with g.mu held (bitmap: m->bitmap.size() bytes)
+int set_mask_locked(hbls_mask* m, const uint8_t* bitmap) {
+    const size_t blen = m->bitmap.size(), n = m->c->n;
+    std::vector<uint8_t> delta(2 * blen + 2, 0);                       // row 0: bits to Add (0 -> 1), row 1: bits to Sub (1 -> 0)
+    bool any = false;
+    for (size_t i = 0; i < n; i++) {                                   // only slots i < n exist (mask.go:121: for i := range m.Publics)
+        const uint8_t msk = (uint8_t)(1u << (i & 7)); const bool was = m->bitmap[i >> 3] & msk, now = bitmap[i >> 3] & msk;
+        if (!was && now) { delta[i >> 3] |= msk; any = true; }
+        if (was && !now) { delta[blen + (i >> 3)] |= msk; any = true; }
+    }
+    if (!any) return 0;
+    Scratch* sc; if (int e = reserve(g.stream, 2 * blen + 4096, &sc)) return e;
+    Arena ar{sc->base, 0, sc->cap};
+    uint8_t* dbm = ar.take<uint8_t>(2 * blen + 2); g1* dtmp = ar.take<g1>(2); int* drc = ar.take<int>(1);
+    CK(cudaMemcpyAsync(dbm, delta.data(), 2 * blen, cudaMemcpyHostToDevice, g.stream));
+    LAUNCH(k_mask_aggregate, 1, 64, g.stream, (size_t)2, n, m->c->table, dbm, blen, dtmp);
+    LAUNCH(k_single, 1, 32, g.stream, (size_t)1, (const single_desc*)nullptr, single_desc{m->d_acc, dtmp + 0, m->d_acc, OP_G1_ADD, 0u}, drc);
+    LAUNCH(k_single, 1, 32, g.stream, (size_t)1, (const single_desc*)nullptr, single_desc{m->d_acc, dtmp + 1, m->d_acc, OP_G1_SUB, 0u}, drc);
+    CK(cudaStreamSynchronize(g.stream));
+    for (size_t i = 0; i < n; i++) {
+        const uint8_t msk = (uint8_t)(1u << (i & 7));
+        m->bitmap[i >> 3] = (uint8_t)((m->bitmap[i >> 3] & ~msk) | (bitmap[i >> 3] & msk));
+    }
     return 0;
 }
 void ensure_stage_events(Scratch* sc) {
@@ -786,7 +951,7 @@ int hbls_hash_prefetch(const void* msg, size_t msg_len) {
     if (!hm_enabled()) return 0;
     if (msg_len > 48) msg_len = 48;
     uint8_t key[48]; hm_key(key, msg, msg_len);
-    for (int i = 0; i < Ctx::HM_N; i++) if (g.hm[i].used && memcmp(g.hm[i].key, key, 48) == 0) { g.hm[i].stamp = ++g.hm_clock; return 0; }
+    if (const int i = hm_find(key); i >= 0) { g.hm[i].stamp = ++g.hm_clock; return 0; }
     cudaStream_t st = g.aux[1];
     Scratch* sc; if (int e = reserve(st, 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};
@@ -796,6 +961,13 @@ int hbls_hash_prefetch(const void* msg, size_t msg_len) {
     launch_hash_small(st, 1, dmsg, 48, dhm, dok);
     hm_store(key, dhm, dok, st);
     CK(cudaGetLastError());
+    return 0;
+}
+int hbls_coalesce_stats(uint64_t* turns, uint64_t* requests, uint64_t* max_turn) {
+    const hbls_coalesce::Stats st = g.part1.stats();
+    if (turns) *turns = st.turns;
+    if (requests) *requests = st.requests;
+    if (max_turn) *max_turn = st.max_turn;
     return 0;
 }
 int hbls_hash_cache_stats(uint64_t* hits, uint64_t* misses) {
@@ -813,90 +985,22 @@ int hbls_get_address(const blsPublicKey* pub, uint8_t out20[20]) {
 void blsGetPublicKey(blsPublicKey* pub, const blsSecretKey* sec) {
     memset(pub, 0, sizeof *pub);
     if (ensure_init()) return;
-    std::lock_guard<std::mutex> lk(g.mu);
-    Scratch* sc; if (reserve(g.stream, 4096, &sc)) return;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dsk = ar.take<uint8_t>(32); g1* dout = ar.take<g1>(1);
-    blsPublicKey tmp;
-    cudaError_t e = cudaMemcpyAsync(dsk, sec->d, 32, cudaMemcpyHostToDevice, g.stream);
-    LAUNCH(k_g1_mul_gen, 1, 32, g.stream, (size_t)1, dsk, dout);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&tmp, dout, 144, cudaMemcpyDeviceToHost, g.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(g.stream);
-    if (e != cudaSuccess) { note_error(e, "blsGetPublicKey", __FILE__, __LINE__); return; }
-    *pub = tmp;
+    Part1Req r; r.kind = RQ_PUBKEY; r.a = sec; r.out = pub;
+    part1_submit(r);
 }
 int blsSignHash(blsSignature* sig, const blsSecretKey* sec, const void* h, size_t size) {
     if (int e = ensure_init()) return e;
-    std::lock_guard<std::mutex> lk(g.mu);
-    if (size > 48) size = 48;
-    Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dsk = ar.take<uint8_t>(32); uint8_t* dmsg = ar.take<uint8_t>(64); g2* dout = ar.take<g2>(1); uint8_t* dok = ar.take<uint8_t>(1);
-    g2a* dhm = ar.take<g2a>(1); uint8_t* dhm_ok = ar.take<uint8_t>(1);
-    CK(cudaMemcpyAsync(dsk, sec->d, 32, cudaMemcpyHostToDevice, g.stream));
-    if (size) CK(cudaMemcpyAsync(dmsg, h, size, cudaMemcpyHostToDevice, g.stream));
     // H(m) on a lane pair (kept in the H(m) cache: the validator verifies the aggregate over the very message it signs here), then
-    // the 255-bit ladder sk * H on the split carrier
-    uint8_t key[48]; bool hit = false;
-    if (hm_enabled()) { hm_key(key, h, size); hit = hm_fetch(key, dhm, dhm_ok, g.stream); }
-    if (!hit) {
-        launch_hash_small(g.stream, 1, dmsg, (uint32_t)size, dhm, dhm_ok);
-        if (hm_enabled()) hm_store(key, dhm, dhm_ok, g.stream);
-    }
-    // sk in base |z| (four 64-bit digits): the ladder runs over psi (kernels.cuh k_sign_hm_gls_pair)
-    uint64_t dig[4];
-    if (sk_digits_base_z(sec->d, dig)) {
-        uint64_t* ddig = ar.take<uint64_t>(4);
-        CK(cudaMemcpyAsync(ddig, dig, sizeof dig, cudaMemcpyHostToDevice, g.stream));
-        LAUNCH(k_sign_hm_gls_pair, 1, 32, g.stream, (size_t)1, ddig, dhm, dhm_ok, (size_t)0, dout, dok);
-    } else
-        LAUNCH(k_sign_hm_pair, 1, 32, g.stream, (size_t)1, dsk, dhm, dhm_ok, (size_t)0, dout, dok);
-    uint8_t ok = 0;
-    CK(cudaMemcpyAsync(sig, dout, 288, cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaMemcpyAsync(&ok, dok, 1, cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return ok ? 0 : -1;
-}
-// VerifyHash on already-decoded structs: d_apk (device Jacobian key) or host pub; returns 1 / 0, <0 on error.  Caller holds g.mu.
-static int verify_hash_locked(const blsSignature* sig, const blsPublicKey* pub, const g1* d_apk, const uint8_t* sig96, const void* h, size_t size) {
-    if (size > 48) size = 48;
-    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(1) + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    VerifyBufs v = carve_verify(ar, 1);
-    g2* dsig = ar.take<g2>(1); uint8_t* dsig96 = ar.take<uint8_t>(96); uint8_t* dmsg = ar.take<uint8_t>(64); uint8_t* dres = ar.take<uint8_t>(1);
-    if (d_apk) CK(cudaMemcpyAsync(v.apk, d_apk, 144, cudaMemcpyDeviceToDevice, g.stream));
-    else CK(cudaMemcpyAsync(v.apk, pub, 144, cudaMemcpyHostToDevice, g.stream));
-    if (size) CK(cudaMemcpyAsync(dmsg, h, size, cudaMemcpyHostToDevice, g.stream));
-    LAUNCH(k_g1_normalize_lat, 1, 32, g.stream, (size_t)1, v.apk, v.pkneg, 1);
-    const uint8_t* ok_sig = nullptr;
-    if (sig96) {          // serialized signature: decode (+ subgroup check) on the device
-        CK(cudaMemcpyAsync(dsig96, sig96, 96, cudaMemcpyHostToDevice, g.stream));
-        LAUNCH(k_g2_decode_pair, 1, 32, g.stream, (size_t)1, dsig96, v.sig, v.ok_sig, 1);
-        ok_sig = v.ok_sig;
-    } else {              // struct inputs are already-decoded Jacobian points: normalise instead of decoding
-        CK(cudaMemcpyAsync(dsig, sig, 288, cudaMemcpyHostToDevice, g.stream));
-        LAUNCH(k_g2_normalize, 1, 32, g.stream, (size_t)1, dsig, v.sig);
-    }
-    {   // H(m): cached when this node has hashed the message before (its own SignHash, a prefetch, an earlier check)
-        uint8_t key[48]; bool hit = false;
-        if (hm_enabled()) { hm_key(key, h, size); hit = hm_fetch(key, v.hm, v.ok_hm, g.stream); }
-        if (!hit) {
-            launch_hash_small(g.stream, 1, dmsg, (uint32_t)size, v.hm, v.ok_hm);
-            if (hm_enabled()) hm_store(key, v.hm, v.ok_hm, g.stream);
-        }
-    }
-    if (g.coop_max >= 1) LAUNCH(k_pairing_coop, 1, 32, g.stream, (size_t)1, v.sig, v.pkneg, v.hm, (const uint8_t*)v.ok_hm, ok_sig, (const uint8_t*)nullptr, dres);
-    else LAUNCH(k_pairing_verify_split, 1, 64, g.stream, (size_t)1, v.sig, v.pkneg, v.hm, (const uint8_t*)v.ok_hm, ok_sig, (const uint8_t*)nullptr, dres, (const int*)nullptr);
-    LAUNCH(k_pairing_fixup, 1, 32, g.stream, (size_t)1, v.sig, v.pkneg, v.hm, (const uint8_t*)v.ok_hm, ok_sig, (const uint8_t*)nullptr, dres, (const int*)nullptr);
-    uint8_t res = 0;
-    CK(cudaMemcpyAsync(&res, dres, 1, cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));
-    return res ? 1 : 0;
+    // the ladder sk * H: over psi with sk in base |z| (kernels.cuh k_sign_hm_gls_pair), else the 255-bit ladder on the split carrier
+    Part1Req r; r.kind = RQ_SIGN; r.a = sec; r.msg = h; r.len = size; r.out = sig;
+    part1_submit(r);
+    return r.err ? r.err : r.rc;
 }
 int blsVerifyHash(const blsSignature* sig, const blsPublicKey* pub, const void* h, size_t size) {
     if (ensure_init()) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
-    return verify_hash_locked(sig, pub, nullptr, nullptr, h, size) == 1 ? 1 : 0;
+    Part1Req r; r.kind = RQ_VERIFY; r.a = sig; r.b = pub; r.msg = h; r.len = size;
+    part1_submit(r);
+    return !r.err && r.rc == 1 ? 1 : 0;
 }
 void blsSign(blsSignature* sig, const blsSecretKey* sec, const void* m, size_t size) {
     uint8_t dg[64]; Sha512::digest((const uint8_t*)m, size, dg);
@@ -1140,36 +1244,17 @@ int hbls_mask_set_mask(hbls_mask* m, const uint8_t* bitmap, size_t blen) {
     if (int e = ensure_init()) return e;
     if (!m || blen != m->bitmap.size()) return HBLS_ERR_ARG;          // mask.go:114-120 "mismatching bitmap lengths"
     std::lock_guard<std::mutex> lk(g.mu);
-    const size_t n = m->c->n;
-    std::vector<uint8_t> delta(2 * blen + 2, 0);                       // row 0: bits to Add (0 -> 1), row 1: bits to Sub (1 -> 0)
-    bool any = false;
-    for (size_t i = 0; i < n; i++) {                                   // only slots i < n exist (mask.go:121: for i := range m.Publics)
-        const uint8_t msk = (uint8_t)(1u << (i & 7)); const bool was = m->bitmap[i >> 3] & msk, now = bitmap[i >> 3] & msk;
-        if (!was && now) { delta[i >> 3] |= msk; any = true; }
-        if (was && !now) { delta[blen + (i >> 3)] |= msk; any = true; }
-    }
-    if (!any) return 0;
-    Scratch* sc; if (int e = reserve(g.stream, 2 * blen + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dbm = ar.take<uint8_t>(2 * blen + 2); g1* dtmp = ar.take<g1>(2); int* drc = ar.take<int>(1);
-    CK(cudaMemcpyAsync(dbm, delta.data(), 2 * blen, cudaMemcpyHostToDevice, g.stream));
-    LAUNCH(k_mask_aggregate, 1, 64, g.stream, (size_t)2, n, m->c->table, dbm, blen, dtmp);
-    LAUNCH(k_single, 1, 32, g.stream, (int)OP_G1_ADD, (const void*)m->d_acc, (const void*)(dtmp + 0), (void*)m->d_acc, drc, 0u);
-    LAUNCH(k_single, 1, 32, g.stream, (int)OP_G1_SUB, (const void*)m->d_acc, (const void*)(dtmp + 1), (void*)m->d_acc, drc, 0u);
-    CK(cudaStreamSynchronize(g.stream));
-    for (size_t i = 0; i < n; i++) {
-        const uint8_t msk = (uint8_t)(1u << (i & 7));
-        m->bitmap[i >> 3] = (uint8_t)((m->bitmap[i >> 3] & ~msk) | (bitmap[i >> 3] & msk));
-    }
-    return 0;
+    return set_mask_locked(m, bitmap);
 }
+// the read-modify-write of the bitmap stays under g.mu: concurrent callers that set different bits keep each other's bits
 int hbls_mask_set_bit(hbls_mask* m, size_t index, int enable) {
+    if (int e = ensure_init()) return e;
     if (!m || index >= m->c->n) return HBLS_ERR_ARG;                   // mask.go:138-140 "index out of range"
-    std::vector<uint8_t> bm;
-    { std::lock_guard<std::mutex> lk(g.mu); bm = m->bitmap; }
+    std::lock_guard<std::mutex> lk(g.mu);
+    std::vector<uint8_t> bm = m->bitmap;
     const uint8_t msk = (uint8_t)(1u << (index & 7));
     if (enable) bm[index >> 3] |= msk; else bm[index >> 3] &= (uint8_t)~msk;
-    return hbls_mask_set_mask(m, bm.data(), bm.size());
+    return set_mask_locked(m, bm.data());
 }
 int hbls_mask_count_enabled(const hbls_mask* m) {
     if (!m) return HBLS_ERR_ARG;
@@ -1195,7 +1280,10 @@ int hbls_mask_verify(const hbls_mask* m, const uint8_t sig96[96], const void* ms
     if (int e = ensure_init()) return e;
     if (!m || !sig96) return HBLS_ERR_ARG;
     std::lock_guard<std::mutex> lk(g.mu);
-    return verify_hash_locked(nullptr, nullptr, m->d_acc, sig96, msg, msg_len);
+    Part1Req r; r.kind = RQ_VERIFY; r.msg = msg; r.len = msg_len;
+    Part1Req* rq = &r;
+    if (int e = part1_locked(&rq, 1, m->d_acc, sig96)) return e;
+    return r.rc;
 }
 int hbls_ballot_box_create(hbls_ballot_box** out, const hbls_committee* c) {
     if (int e = ensure_init()) return e;
@@ -1219,7 +1307,7 @@ int hbls_ballot_box_add_vote(hbls_ballot_box* b, const uint8_t* signer_bitmap, s
     Arena ar{sc->base, 0, sc->cap};
     uint8_t* dsig = ar.take<uint8_t>(96); int* drc = ar.take<int>(1);
     CK(cudaMemcpyAsync(dsig, sig96, 96, cudaMemcpyHostToDevice, g.stream));
-    LAUNCH(k_single, 1, 32, g.stream, (int)OP_G2_DES_ADD, (const void*)dsig, (const void*)nullptr, (void*)b->d_sum, drc, 0u);
+    LAUNCH(k_single, 1, 32, g.stream, (size_t)1, (const single_desc*)nullptr, single_desc{dsig, nullptr, b->d_sum, OP_G2_DES_ADD, 0u}, drc);
     int rc = 0;
     CK(cudaMemcpyAsync(&rc, drc, sizeof(int), cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));

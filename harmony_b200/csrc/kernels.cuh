@@ -414,10 +414,12 @@ __global__ void __launch_bounds__(32) k_hash_to_g2_coop(size_t n, const uint8_t*
 }
 
 // same-message batches (the leader's prepare / commit vote collection, consensus/leader.go:127-290: every vote signs
-// the same block hash / commit payload): H(m) is computed once and replicated
-__global__ void k_broadcast_hm(size_t n, g2a* hm, uint8_t* ok) {
-    size_t i = HB_TID; if (i == 0 || i >= n) return;
-    hm[i] = hm[0]; ok[i] = ok[0];
+// the same block hash / commit payload): H(m) is computed once and replicated.  With an index (concurrent herumi-API calls
+// combined into one turn, hbls.cu): H(m) of each distinct message once, gathered to the requests -- hm[i] = src[idx[i]].
+__global__ void k_broadcast_hm(size_t n, const uint32_t* idx, const g2a* src, const uint8_t* src_ok, g2a* hm, uint8_t* ok) {
+    size_t i = HB_TID; if (i >= n) return;
+    if (!idx) { if (i == 0) return; hm[i] = hm[0]; ok[i] = ok[0]; }
+    else { hm[i] = src[idx[i]]; ok[i] = src_ok[idx[i]]; }
 }
 
 // ---- verification (R7/R8)
@@ -1160,13 +1162,15 @@ __global__ void k_sign_hm_gls_pair(size_t n, const uint64_t* digits, const g2a* 
     if ((threadIdx.x & 1) == 0) { out[i] = r; ok[i] = good ? 1 : 0; }
 }
 
-// ---- single-element ops behind the herumi-shaped C ABI (one thread; latency is launch-bound)
+// ---- single-element ops behind the herumi-shaped C ABI (one thread per op; latency is launch-bound)
 enum { OP_G1_ADD = 1, OP_G1_SUB, OP_G2_ADD, OP_G1_EQ, OP_G2_EQ, OP_G1_SER, OP_G2_SER, OP_G1_DES, OP_G2_DES, OP_MAP_SER, OP_G2_DES_ADD };
-__global__ void k_single(int op, const void* a, const void* b, void* out, int* rc, uint32_t len) {
-    if (HB_TID != 0) return;
-    switch (op) {
+// one op: device operands a, b (nullable), result out, message length len (OP_MAP_SER)
+struct single_desc { const void* a; const void* b; void* out; int op; uint32_t len; };
+HB_DEV void run_single(const single_desc& s, int* rc) {
+    const void* a = s.a; const void* b = s.b; void* out = s.out;
+    switch (s.op) {
     case OP_G1_ADD: case OP_G1_SUB: {
-        g1 x = *(const g1*)a, y = *(const g1*)b; if (op == OP_G1_SUB) pt_neg(y, y);
+        g1 x = *(const g1*)a, y = *(const g1*)b; if (s.op == OP_G1_SUB) pt_neg(y, y);
         pt_add(x, x, y); *(g1*)out = x; *rc = 0; break; }
     case OP_G2_ADD: { g2 x = *(const g2*)a, y = *(const g2*)b; pt_add(x, x, y); *(g2*)out = x; *rc = 0; break; }
     case OP_G1_EQ: { g1 x = *(const g1*)a, y = *(const g1*)b; *rc = pt_eq(x, y) ? 1 : 0; break; }
@@ -1175,13 +1179,18 @@ __global__ void k_single(int op, const void* a, const void* b, void* out, int* r
     case OP_G2_SER: { g2 x = *(const g2*)a; g2_serialize((uint8_t*)out, x); *rc = 96; break; }
     case OP_G1_DES: { g1 x; bool g = g1_deserialize(x, (const uint8_t*)a, true); if (g) *(g1*)out = x; *rc = g ? 48 : 0; break; }
     case OP_G2_DES: { g2 x; bool g = g2_deserialize(x, (const uint8_t*)a, true); if (g) *(g2*)out = x; *rc = g ? 96 : 0; break; }
-    case OP_MAP_SER: { g2 h; bool g = map_to_g2(h, (const uint8_t*)a, len); if (g) g2_serialize((uint8_t*)out, h); *rc = g ? 0 : -1; break; }
+    case OP_MAP_SER: { g2 h; bool g = map_to_g2(h, (const uint8_t*)a, s.len); if (g) g2_serialize((uint8_t*)out, h); *rc = g ? 0 : -1; break; }
     case OP_G2_DES_ADD: {   // ballot box: out (Jacobian running sum) += decode(a); rc = 96 ok / 0 undecodable (sum untouched)
         g2 x; bool g = g2_deserialize(x, (const uint8_t*)a, true);
         if (g) { g2 acc = *(const g2*)out; pt_add(acc, acc, x); *(g2*)out = acc; }
         *rc = g ? 96 : 0; break; }
     default: *rc = -1;
     }
+}
+// thread i runs op i: ops[i] (device array), or `one` when ops is null (n = 1, nothing to stage); rc[i] its return code
+__global__ void k_single(size_t n, const single_desc* ops, single_desc one, int* rc) {
+    const size_t i = HB_TID; if (i >= n) return;
+    run_single(ops ? ops[i] : one, rc + i);
 }
 
 // ---- integer-pipe roofline probe: K independent accumulator sets per thread, each fed by lane_mad -- the exact

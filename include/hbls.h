@@ -11,8 +11,12 @@
  *     internal/chain/engine.go:619-642 verifySignature, consensus/leader.go:227-290 onCommit loop).
  *
  * Conventions: plain pointers and sizes only; all memory caller-owned; no callbacks; int error codes.
- * Threading: every function may be called from any thread after blsInit; calls are serialised by one library mutex and
- * (except hbls_aggregate_verify_batch_device on a caller stream) one library stream.  Scratch memory is per stream, so
+ * Threading: every function may be called from any thread after blsInit.  Part-1 calls made concurrently (VerifyHash / Verify,
+ * SignHash / Sign, GetPublicKey, Add / Sub, IsEqual, Serialize / Deserialize of keys and signatures, hbls_map_to_g2) are combined
+ * into shared device launches: while one turn runs on the GPU, or a batch call holds it, the calls that arrive queue up and the next
+ * caller in line runs them all as one turn (hbls_coalesce_stats counts the turns).  There is no timer or batching window: a call
+ * that finds the library idle runs at once, alone, with the launches it has always made.  Device work is serialised by one library
+ * mutex and (except hbls_aggregate_verify_batch_device on a caller stream) one library stream.  Scratch memory is per stream, so
  * asynchronous device-pointer calls on DIFFERENT streams do not share intermediates; calls on one stream are stream-ordered.
  * Messages: only the first min(len, 48) bytes enter the map to G2 (mcl setArrayMask; SURVEY A.3); batch entry points take the
  * message stride msg_len and read min(msg_len, 48) bytes per item.
@@ -238,6 +242,9 @@ int hbls_get_public_key_batch(size_t k, const uint8_t* sk32, uint8_t* pk48_out);
  * id -- hence the commit payload -- become known).  hbls_set_param("hm_cache", 0) turns the cache off.  0 ok. */
 int hbls_hash_prefetch(const void* msg, size_t msg_len);
 int hbls_hash_cache_stats(uint64_t* hits, uint64_t* misses);
+/* Part-1 calls combined so far (include/hbls.h: threading): turns run, requests served by them and the largest turn.  A process
+ * whose herumi-API calls never overlap sees turns == requests and max_turn == 1.  Each pointer is nullable.  0 ok. */
+int hbls_coalesce_stats(uint64_t* turns, uint64_t* requests, uint64_t* max_turn);
 
 /* ------------------------------------------------------------------ probes used by tests / bench */
 /* message -> G2 point, serialized (the H(m) of SignHash/VerifyHash): 0 ok, -1 undefined */
