@@ -21,7 +21,7 @@ _COMPILED_TIME_VAR = 46
 PublicKeySizeInBytes = 48
 BLSSignatureSizeInBytes = 96
 
-ERR_CUDA, ERR_ARG, ERR_DECODE = -100, -2, -3
+ERR_CUDA, ERR_ARG, ERR_DECODE, ERR_SELF_TEST = -100, -2, -3, -4
 
 _lib = None
 _inited = False
@@ -35,6 +35,10 @@ class BatchInfo(ctypes.Structure):
                 ("groups_failed", ctypes.c_uint32), ("rounds_rechecked", ctypes.c_uint32), ("tail_rounds", ctypes.c_uint32),
                 ("cta_threads", ctypes.c_uint32)]
     def as_dict(self): return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+class SelfTestReport(ctypes.Structure):
+    """hbls_self_test_report (include/hbls.h)."""
+    _fields_ = [("failed_legs", ctypes.c_uint64), ("legs", ctypes.c_uint32), ("kernels", ctypes.c_uint32), ("ms", ctypes.c_float)]
 
 class _Sec(ctypes.Structure):
     _fields_ = [("d", ctypes.c_uint64 * 4)]
@@ -121,6 +125,9 @@ def lib():
         sig("hbls_coalesce_stats", c.c_int, c.POINTER(c.c_uint64), c.POINTER(c.c_uint64), c.POINTER(c.c_uint64))
         sig("hbls_stage_timing_enable", None, c.c_int)
         sig("hbls_stage_timing_get", c.c_int, c.POINTER(c.c_float), c.c_int)
+        sig("hbls_self_test", c.c_int, c.POINTER(SelfTestReport))
+        sig("hbls_self_test_leg_name", c.c_int, c.c_int, vp, sz)
+        sig("hbls_self_test_kernels", c.c_int, vp, sz)
         _lib = L
     return _lib
 
@@ -464,6 +471,25 @@ def ConstructCommitPayload(is_staking: bool, block_hash: bytes, block_num: int, 
     out = block_num.to_bytes(8, "little") + bytes(block_hash)
     if is_staking: out += view_id.to_bytes(8, "little")
     return out
+
+def SelfTestLegName(leg: int) -> str:
+    buf = ctypes.create_string_buffer(64)
+    if lib().hbls_self_test_leg_name(leg, buf, 64) != 0: raise ValueError(f"no self-test leg {leg}")
+    return buf.value.decode()
+def SelfTestKernels():
+    """names of the distinct kernels the last self-test launched"""
+    n = lib().hbls_self_test_kernels(None, 0)
+    buf = ctypes.create_string_buffer(n + 1)
+    lib().hbls_self_test_kernels(buf, n + 1)
+    return buf.value.decode().split()
+def SelfTest() -> dict:
+    """hbls_self_test: every kernel of the library on inputs with built-in known answers.  Returns the report with the names of the
+    failed legs ("failed": [] when everything passes); raises HblsError when the test could not run."""
+    rep = SelfTestReport()
+    rc = _need().hbls_self_test(ctypes.byref(rep))
+    if rc < 0: raise HblsError(f"hbls_self_test rc={rc}")
+    failed = [SelfTestLegName(i) for i in range(rep.legs) if rep.failed_legs >> i & 1]
+    return {"rc": rc, "failed_legs": int(rep.failed_legs), "legs": int(rep.legs), "kernels": int(rep.kernels), "ms": float(rep.ms), "failed": failed}
 
 def SelfTestSplit(iters: int = 16) -> int: return int(_need().hbls_selftest_split(iters))
 def SetBatchMode(mode: int): lib().hbls_set_batch_mode(int(mode))

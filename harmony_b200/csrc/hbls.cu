@@ -10,6 +10,8 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <set>
+#include <string>
 #include <vector>
 #include "../../include/hbls.h"
 #include "coalesce.hpp"
@@ -59,6 +61,9 @@ struct Ctx {
     uint64_t hm_clock = 0, hm_hits = 0, hm_misses = 0;
     long long hm_cache = 1;                                 // hbls_set_param("hm_cache", 0) turns it off (cold-path measurements)
     hbls_coalesce::Combiner part1;                          // concurrent herumi-API calls (include/hbls.h part 1) -> shared turns
+    // built-in self-test (selftest.cuh): kernels launched by the last run, a failed run at init disables the library
+    bool st_rec = false, st_failed = false; std::set<std::string> st_kernels;
+    long long selftest_flip = 0;                            // test hook: leg + 1 whose expected answer the next run flips
 };
 Ctx g;
 
@@ -70,6 +75,7 @@ void note_error(cudaError_t e, const char* what, const char* file, int line) {
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { note_error(e_, #call, __FILE__, __LINE__); return HBLS_ERR_CUDA; } } while (0)
 
 int ensure_init() {
+    if (g.st_failed) { fprintf(stderr, "[hbls] the self-test failed at initialisation: the library refuses all work\n"); return HBLS_ERR_SELF_TEST; }
     if (g.ready) return 0;
     fprintf(stderr, "[hbls] not initialised: call blsInit / hbls_init_device first (no CPU fallback)\n");
     return HBLS_ERR_CUDA;
@@ -141,8 +147,10 @@ void hm_store(const uint8_t key[48], const g2a* src, const uint8_t* src_ok, cuda
     cudaEventRecord(e.filled, st);
     memcpy(e.key, key, 48); e.used = true; e.has_reader = false; e.stamp = ++g.hm_clock;
 }
-#define LAUNCH(kern, grid, block, strm, ...) do { kern<<<(grid), (block), 0, (strm)>>>(__VA_ARGS__); g.launches++; } while (0)
-#define LAUNCH_SMEM(kern, grid, block, smem, strm, ...) do { kern<<<(grid), (block), (smem), (strm)>>>(__VA_ARGS__); g.launches++; } while (0)
+// while the self-test runs, every launch records its kernel's name (hbls_self_test_kernels)
+#define ST_NOTE(kern) do { if (g.st_rec) g.st_kernels.insert(#kern); } while (0)
+#define LAUNCH(kern, grid, block, strm, ...) do { kern<<<(grid), (block), 0, (strm)>>>(__VA_ARGS__); g.launches++; ST_NOTE(kern); } while (0)
+#define LAUNCH_SMEM(kern, grid, block, smem, strm, ...) do { kern<<<(grid), (block), (smem), (strm)>>>(__VA_ARGS__); g.launches++; ST_NOTE(kern); } while (0)
 
 constexpr unsigned TPB = 64;      // heavy kernels: 64-thread CTAs
 // persistent launch geometry for the grid-stride kernels: at most `tpsm` resident threads per SM (default 384) so the per-thread
@@ -161,6 +169,20 @@ unsigned split_blocks(size_t nthreads) { return capped_blocks(nthreads, g.tpsm_s
 void launch_hash_small(cudaStream_t st, size_t n, const uint8_t* d_msgs, uint32_t msg_len, g2a* hm, uint8_t* ok_hm) {
     if ((long long)n <= g.hash_coop_max) LAUNCH(k_hash_to_g2_coop, (unsigned)n, 32, st, n, d_msgs, msg_len, hm, ok_hm, (int)g.hash_fallback);
     else LAUNCH(k_hash_to_g2_pair, blocks_for(2 * n, 32), 32, st, n, d_msgs, msg_len, hm, ok_hm);
+}
+
+// hash-to-G2 of a large batch, one message per thread: one kernel, or map + cofactor clearing (hash_split 1), or map + cofactor
+// clearing into the Jacobian buffer S (B points) + affine conversion (hash_split 2)
+void launch_hash_batch(cudaStream_t s, size_t B, const uint8_t* d_msgs, uint32_t msg_len, g2a* hm, uint8_t* ok_hm, g2* S) {
+    if (g.hash_split && HB_BATCH_INV) {
+        LAUNCH(k_hash_sw, capped_blocks(B, g.tpsm_sw, TPB), TPB, s, B, d_msgs, msg_len, hm, ok_hm);
+        if (g.hash_split >= 2) {        // three kernels: map | cofactor clearing (Jacobian, into the S buffer the scaling stage fills later) | affine
+            LAUNCH(k_hash_cofactor_jac, capped_blocks(B, g.tpsm_cof, TPB), TPB, s, B, (const g2a*)hm, (const uint8_t*)ok_hm, S);
+            LAUNCH(k_g2_normalize_batch, heavy_blocks(B), TPB, s, B, (const g2*)S, hm);
+        } else
+            LAUNCH(k_hash_cofactor, heavy_blocks(B), TPB, s, B, hm, (const uint8_t*)ok_hm);
+    } else
+        LAUNCH(k_hash_to_g2, heavy_blocks(B), TPB, s, B, d_msgs, msg_len, hm, ok_hm);
 }
 
 // ------------------------------------------------------------------ coefficient stream (host): ChaCha20 block function, RFC 8439
@@ -309,15 +331,8 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
         if (B > 1) LAUNCH(k_broadcast_hm, blocks_for(B, 256), 256, sh, B, (const uint32_t*)nullptr, (const g2a*)v.hm, (const uint8_t*)v.ok_hm, v.hm, v.ok_hm);
     } else if (pairs)
         launch_hash_small(sh, B, d_msgs, msg_len, v.hm, v.ok_hm);
-    else if (g.hash_split && HB_BATCH_INV) {
-        LAUNCH(k_hash_sw, capped_blocks(B, g.tpsm_sw, TPB), TPB, s, B, d_msgs, msg_len, v.hm, v.ok_hm);
-        if (g.hash_split >= 2) {        // three kernels: map | cofactor clearing (Jacobian, into the S buffer the scaling stage fills later) | affine
-            LAUNCH(k_hash_cofactor_jac, capped_blocks(B, g.tpsm_cof, TPB), TPB, s, B, (const g2a*)v.hm, (const uint8_t*)v.ok_hm, v.S);
-            LAUNCH(k_g2_normalize_batch, heavy_blocks(B), TPB, s, B, (const g2*)v.S, v.hm);
-        } else
-            LAUNCH(k_hash_cofactor, heavy_blocks(B), TPB, s, B, v.hm, (const uint8_t*)v.ok_hm);
-    } else
-        LAUNCH(k_hash_to_g2, heavy_blocks(B), TPB, s, B, d_msgs, msg_len, v.hm, v.ok_hm);
+    else
+        launch_hash_batch(s, B, d_msgs, msg_len, v.hm, v.ok_hm, v.S);
     if (warm) {
         cudaEventRecord(sc->join[1], sh); cudaStreamWaitEvent(s, sc->join[1], 0);
         LAUNCH(k_miller_pq_coop, coop_grid, 32, s, B, (const g1a*)v.pkneg, v.hm, (const uint8_t*)v.ok_hm, v.f2, v.irr2);
@@ -733,6 +748,19 @@ bool all_messages_equal(const uint8_t* msgs, size_t n, size_t msg_len) {
     for (size_t i = 1; i < n; i++) if (memcmp(msgs, msgs + i * msg_len, msg_len) != 0) return false;
     return n > 1;
 }
+// serial mask aggregation of large batches: rounds sorted by the number of point additions they need (device counting sort, when
+// mask_sort is on), so that the lanes of a warp finish together; v.apk receives the Jacobian sums
+void launch_mask_serial(const hbls_committee* c, size_t B, const uint8_t* d_bitmaps, size_t blen, const VerifyBufs& v, cudaStream_t s) {
+    const uint32_t* order = nullptr;
+    if (g.mask_sort && B <= 0xffffffffull) {
+        cudaMemsetAsync(v.mask_hist, 0, HB_MASK_BINS * sizeof(unsigned), s);
+        LAUNCH(k_mask_count, blocks_for(B, 256), 256, s, B, c->n, d_bitmaps, blen, v.mask_cost, v.mask_hist);
+        LAUNCH(k_mask_scan, 1, 32, s, v.mask_hist);
+        LAUNCH(k_mask_scatter, blocks_for(B, 256), 256, s, B, v.mask_cost, v.mask_hist, v.mask_order);
+        order = v.mask_order;
+    }
+    LAUNCH(k_mask_aggregate_serial, light_blocks(B), TPB, s, B, c->n, c->table, c->total, d_bitmaps, blen, v.apk, order);
+}
 // rounds against one committee, everything device-resident
 int agg_verify_device_locked(const hbls_committee* c, size_t B, const uint8_t* d_bitmaps, size_t blen, const uint8_t* d_sigs,
                              const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, Arena& ar, bool same_msg,
@@ -741,18 +769,7 @@ int agg_verify_device_locked(const hbls_committee* c, size_t B, const uint8_t* d
     fork_point(B, sc, s);
     STAGE_EV(0, sc, s);
     if (B >= (size_t)g.sm_count * 256)
-    {
-        // rounds sorted by the number of point additions they need (device counting sort), so that the lanes of a warp finish together
-        const uint32_t* order = nullptr;
-        if (g.mask_sort && B <= 0xffffffffull) {
-            cudaMemsetAsync(v.mask_hist, 0, HB_MASK_BINS * sizeof(unsigned), s);
-            LAUNCH(k_mask_count, blocks_for(B, 256), 256, s, B, c->n, d_bitmaps, blen, v.mask_cost, v.mask_hist);
-            LAUNCH(k_mask_scan, 1, 32, s, v.mask_hist);
-            LAUNCH(k_mask_scatter, blocks_for(B, 256), 256, s, B, v.mask_cost, v.mask_hist, v.mask_order);
-            order = v.mask_order;
-        }
-        LAUNCH(k_mask_aggregate_serial, light_blocks(B), TPB, s, B, c->n, c->table, c->total, d_bitmaps, blen, v.apk, order);
-    }
+        launch_mask_serial(c, B, d_bitmaps, blen, v, s);
     else
         LAUNCH(k_mask_aggregate, blocks_for(B * 32, 128), 128, s, B, c->n, c->table, d_bitmaps, blen, v.apk);
     launch_verify_tail(B, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, same_msg, h_msg);
@@ -789,10 +806,13 @@ void ensure_stage_events(Scratch* sc) {
 }
 }  // namespace
 
+int self_test_at_init();      // selftest.cuh: HBLS_SELF_TEST=1 runs hbls_self_test here
+
 extern "C" {
 
 int hbls_init_device(int device) {
     std::lock_guard<std::mutex> lk(g.mu);
+    if (g.st_failed) return HBLS_ERR_SELF_TEST;
     if (g.ready) return 0;
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);
@@ -843,7 +863,7 @@ int hbls_init_device(int device) {
     CK(cudaFuncSetAttribute(k_hash_cofactor_jac, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_g2_normalize_batch, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     g.ready = true;
-    return 0;
+    return self_test_at_init();
 }
 int blsInit(int curve, int compiledTimeVar) {
     if (curve != HBLS_BLS12_381 || compiledTimeVar != HBLS_COMPILED_TIME_VAR) return -1;
@@ -855,32 +875,17 @@ uint64_t hbls_kernel_launch_count(void) { return g.launches.load(); }
 int hbls_build_info(void) { return (HB_BATCH_INV ? 1 : 0) | (HB_BATCH_K << 8); }
 void hbls_set_batch_mode(int mode) { std::lock_guard<std::mutex> lk(g.mu); g.batch_mode = mode ? 1 : 0; }
 int hbls_get_batch_mode(void) { std::lock_guard<std::mutex> lk(g.mu); return g.batch_mode; }
+// tuning knobs by name (hbls_set_param); the self-test saves and restores all of them
+struct ParamDef { const char* name; long long Ctx::* slot; };
+const ParamDef PARAMS[] = {
+    {"rlc_min", &Ctx::rlc_min}, {"rlc_g", &Ctx::rlc_g}, {"tpsm", &Ctx::tpsm}, {"tpsm_split", &Ctx::tpsm_split}, {"tpsm_light", &Ctx::tpsm_light}, {"coop_max", &Ctx::coop_max},
+    {"overlap", &Ctx::overlap}, {"coop_wpsm", &Ctx::coop_wpsm}, {"hm_cache", &Ctx::hm_cache}, {"hash_coop_max", &Ctx::hash_coop_max}, {"mask_sort", &Ctx::mask_sort}, {"hash_split", &Ctx::hash_split},
+    {"hash_fallback", &Ctx::hash_fallback}, {"rlc_two_phase", &Ctx::rlc_two_phase}, {"tpsm_cof", &Ctx::tpsm_cof}, {"tpsm_dec", &Ctx::tpsm_dec}, {"tpsm_scale", &Ctx::tpsm_scale}, {"tpsm_scale_g1", &Ctx::tpsm_scale_g1},
+    {"scale_split", &Ctx::scale_split}, {"decode_split", &Ctx::decode_split}, {"exact_two_phase", &Ctx::exact_two_phase}, {"tpsm_lines", &Ctx::tpsm_lines}, {"tpsm_accum", &Ctx::tpsm_accum}, {"tpsm_sw", &Ctx::tpsm_sw},
+    {"selftest_flip", &Ctx::selftest_flip}};
 static long long* param_slot(const char* name) {
     if (!name) return nullptr;
-    if (!strcmp(name, "rlc_min")) return &g.rlc_min;
-    if (!strcmp(name, "rlc_g")) return &g.rlc_g;
-    if (!strcmp(name, "tpsm")) return &g.tpsm;
-    if (!strcmp(name, "tpsm_split")) return &g.tpsm_split;
-    if (!strcmp(name, "tpsm_light")) return &g.tpsm_light;
-    if (!strcmp(name, "coop_max")) return &g.coop_max;
-    if (!strcmp(name, "overlap")) return &g.overlap;
-    if (!strcmp(name, "coop_wpsm")) return &g.coop_wpsm;
-    if (!strcmp(name, "hm_cache")) return &g.hm_cache;
-    if (!strcmp(name, "hash_coop_max")) return &g.hash_coop_max;
-    if (!strcmp(name, "mask_sort")) return &g.mask_sort;
-    if (!strcmp(name, "hash_split")) return &g.hash_split;
-    if (!strcmp(name, "hash_fallback")) return &g.hash_fallback;
-    if (!strcmp(name, "rlc_two_phase")) return &g.rlc_two_phase;
-    if (!strcmp(name, "tpsm_cof")) return &g.tpsm_cof;
-    if (!strcmp(name, "tpsm_dec")) return &g.tpsm_dec;
-    if (!strcmp(name, "tpsm_scale")) return &g.tpsm_scale;
-    if (!strcmp(name, "tpsm_scale_g1")) return &g.tpsm_scale_g1;
-    if (!strcmp(name, "scale_split")) return &g.scale_split;
-    if (!strcmp(name, "decode_split")) return &g.decode_split;
-    if (!strcmp(name, "exact_two_phase")) return &g.exact_two_phase;
-    if (!strcmp(name, "tpsm_lines")) return &g.tpsm_lines;
-    if (!strcmp(name, "tpsm_accum")) return &g.tpsm_accum;
-    if (!strcmp(name, "tpsm_sw")) return &g.tpsm_sw;
+    for (const ParamDef& p : PARAMS) if (!strcmp(name, p.name)) return &(g.*p.slot);
     return nullptr;
 }
 int hbls_set_param(const char* name, long long value) {
@@ -909,6 +914,7 @@ int hbls_last_batch_info(hbls_batch_info* out) {
 
 // ------------------------------------------------------------------ secret keys (host bytes; no group arithmetic)
 int blsSecretKeySetByCSPRNG(blsSecretKey* sec) {
+    if (g.st_failed) return -1;
     FILE* f = fopen("/dev/urandom", "rb");
     if (!f) return -1;
     size_t got = fread(sec->d, 1, 32, f); fclose(f);
@@ -916,14 +922,14 @@ int blsSecretKeySetByCSPRNG(blsSecretKey* sec) {
     sec->d[3] &= 0x3fffffffffffffffull;          // < 2^254 < r
     return 0;
 }
-size_t blsSecretKeySerialize(void* buf, size_t maxBufSize, const blsSecretKey* sec) { if (maxBufSize < 32) return 0; memcpy(buf, sec->d, 32); return 32; }
+size_t blsSecretKeySerialize(void* buf, size_t maxBufSize, const blsSecretKey* sec) { if (maxBufSize < 32 || g.st_failed) return 0; memcpy(buf, sec->d, 32); return 32; }
 size_t blsSecretKeyDeserialize(blsSecretKey* sec, const void* buf, size_t bufSize) {
-    if (bufSize < 32) return 0;
+    if (bufSize < 32 || g.st_failed) return 0;
     uint64_t k[4]; memcpy(k, buf, 32);
     if (!scalar_lt_r(k)) return 0;
     memcpy(sec->d, k, 32); return 32;
 }
-int blsSecretKeyIsEqual(const blsSecretKey* l, const blsSecretKey* r) { return memcmp(l, r, 32) == 0; }
+int blsSecretKeyIsEqual(const blsSecretKey* l, const blsSecretKey* r) { return !g.st_failed && memcmp(l, r, 32) == 0; }
 
 // ------------------------------------------------------------------ single-element group ops.  The herumi signatures of Add / Sub /
 // GetPublicKey are void: on a CUDA failure the destination becomes the identity and the error is kept for hbls_last_error().
@@ -1012,10 +1018,7 @@ int blsVerify(const blsSignature* sig, const blsPublicKey* pub, const void* m, s
 }
 
 // ------------------------------------------------------------------ committee table
-int hbls_committee_create(hbls_committee** out, const uint8_t* pk48, size_t n, size_t* bad_index) {
-    if (int e = ensure_init()) return e;
-    if (!out) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+static int committee_create_locked(hbls_committee** out, const uint8_t* pk48, size_t n, size_t* bad_index) {
     std::unique_ptr<hbls_committee> c(new hbls_committee); c->n = n;       // freed (with its device tables) on every early return
     size_t nn = n ? n : 1;
     CK(cudaMalloc(&c->table, nn * sizeof(g1a)));
@@ -1034,13 +1037,16 @@ int hbls_committee_create(hbls_committee** out, const uint8_t* pk48, size_t n, s
     for (size_t i = 0; i < n; i++) if (!ok[i]) { if (bad_index) *bad_index = i; return HBLS_ERR_DECODE; }
     *out = c.release(); return 0;
 }
+int hbls_committee_create(hbls_committee** out, const uint8_t* pk48, size_t n, size_t* bad_index) {
+    if (int e = ensure_init()) return e;
+    if (!out) return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return committee_create_locked(out, pk48, n, bad_index);
+}
 void hbls_committee_destroy(hbls_committee* c) { if (!c) return; std::lock_guard<std::mutex> lk(g.mu); cudaDeviceSynchronize(); delete c; }
 size_t hbls_committee_size(const hbls_committee* c) { return c ? c->n : 0; }
 
-int hbls_mask_aggregate(const hbls_committee* c, const uint8_t* bitmap, size_t blen, uint8_t out_pk48[48]) {
-    if (int e = ensure_init()) return e;
-    if (!c || blen != ((c->n + 7) >> 3)) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+static int mask_aggregate_locked(const hbls_committee* c, const uint8_t* bitmap, size_t blen, uint8_t out_pk48[48]) {
     Scratch* sc; if (int e = reserve(g.stream, blen + 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};
     uint8_t* dbm = ar.take<uint8_t>(blen ? blen : 1); g1* dacc = ar.take<g1>(1); uint8_t* dout = ar.take<uint8_t>(48);
@@ -1051,10 +1057,14 @@ int hbls_mask_aggregate(const hbls_committee* c, const uint8_t* bitmap, size_t b
     CK(cudaStreamSynchronize(g.stream));
     return 0;
 }
-
-int hbls_aggregate_sigs(const uint8_t* sig96, size_t n, uint8_t out96[96]) {
+int hbls_mask_aggregate(const hbls_committee* c, const uint8_t* bitmap, size_t blen, uint8_t out_pk48[48]) {
     if (int e = ensure_init()) return e;
+    if (!c || blen != ((c->n + 7) >> 3)) return HBLS_ERR_ARG;
     std::lock_guard<std::mutex> lk(g.mu);
+    return mask_aggregate_locked(c, bitmap, blen, out_pk48);
+}
+
+static int aggregate_sigs_locked(const uint8_t* sig96, size_t n, uint8_t out96[96]) {
     size_t nn = n ? n : 1;
     Scratch* sc; if (int e = reserve(g.stream, nn * (96 + sizeof(g2a) + 1) + 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};
@@ -1072,6 +1082,11 @@ int hbls_aggregate_sigs(const uint8_t* sig96, size_t n, uint8_t out96[96]) {
     CK(cudaStreamSynchronize(g.stream));
     for (size_t i = 0; i < n; i++) if (!ok[i]) return HBLS_ERR_DECODE;
     return 0;
+}
+int hbls_aggregate_sigs(const uint8_t* sig96, size_t n, uint8_t out96[96]) {
+    if (int e = ensure_init()) return e;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return aggregate_sigs_locked(sig96, n, out96);
 }
 
 // ------------------------------------------------------------------ aggregate verification
@@ -1126,12 +1141,8 @@ int hbls_aggregate_verify(const hbls_committee* c, const uint8_t* bitmap, size_t
     if (rc) return rc;
     return res ? 1 : 0;
 }
-int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96, const uint8_t* bitmaps, size_t blen,
+static int verify_headers_locked(const hbls_committee* c, size_t n, const uint8_t* sigs96, const uint8_t* bitmaps, size_t blen,
                         const uint8_t* payloads, size_t payload_len, size_t quorum, uint8_t* status) {
-    if (int e = ensure_init()) return e;
-    if (!c || blen != ((c->n + 7) >> 3) || !status) return HBLS_ERR_ARG;        // DecodeSigBitmap: mask.SetMask length error (sig.go:43)
-    if (n == 0) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
     std::vector<uint8_t> res(n), flags(n);
     if (int e = agg_verify_host_locked(c, n, bitmaps, blen, sigs96, payloads, payload_len, res.data(), flags.data())) return e;
     for (size_t i = 0; i < n; i++) {
@@ -1142,15 +1153,19 @@ int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96
     }
     return 0;
 }
-
-int hbls_aggregate_verify_items(size_t k, const hbls_committee* const* committees, const uint8_t* bitmaps, const uint8_t* sigs96,
-                                const uint8_t* msgs, size_t msg_len, uint8_t* results) {
+int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96, const uint8_t* bitmaps, size_t blen,
+                        const uint8_t* payloads, size_t payload_len, size_t quorum, uint8_t* status) {
     if (int e = ensure_init()) return e;
-    if (k == 0) return 0;
-    if (!committees || !results) return HBLS_ERR_ARG;
-    size_t bm_bytes = 0;
-    for (size_t j = 0; j < k; j++) { if (!committees[j]) return HBLS_ERR_ARG; bm_bytes += (committees[j]->n + 7) >> 3; }
+    if (!c || blen != ((c->n + 7) >> 3) || !status) return HBLS_ERR_ARG;        // DecodeSigBitmap: mask.SetMask length error (sig.go:43)
+    if (n == 0) return 0;
     std::lock_guard<std::mutex> lk(g.mu);
+    return verify_headers_locked(c, n, sigs96, bitmaps, blen, payloads, payload_len, quorum, status);
+}
+
+static int aggregate_verify_items_locked(size_t k, const hbls_committee* const* committees, const uint8_t* bitmaps, const uint8_t* sigs96,
+                                const uint8_t* msgs, size_t msg_len, uint8_t* results) {
+    size_t bm_bytes = 0;
+    for (size_t j = 0; j < k; j++) bm_bytes += (committees[j]->n + 7) >> 3;
     Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(k) + bm_bytes + k * (96 + msg_len + 1 + sizeof(mask_item)) + 4096, &sc)) return e;
     ensure_stage_events(sc);
     Arena ar{sc->base, 0, sc->cap};
@@ -1170,6 +1185,15 @@ int hbls_aggregate_verify_items(size_t k, const hbls_committee* const* committee
     CK(cudaMemcpyAsync(results, dres, k, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));          // items[] (pageable source of an async copy) stays alive until here
     return 0;
+}
+int hbls_aggregate_verify_items(size_t k, const hbls_committee* const* committees, const uint8_t* bitmaps, const uint8_t* sigs96,
+                                const uint8_t* msgs, size_t msg_len, uint8_t* results) {
+    if (int e = ensure_init()) return e;
+    if (k == 0) return 0;
+    if (!committees || !results) return HBLS_ERR_ARG;
+    for (size_t j = 0; j < k; j++) if (!committees[j]) return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return aggregate_verify_items_locked(k, committees, bitmaps, sigs96, msgs, msg_len, results);
 }
 
 // shared body of hbls_verify_batch / hbls_verify_batch_status; flags_out (nullable): k_pack_flags bytes per item
@@ -1204,11 +1228,7 @@ int hbls_verify_batch(size_t k, const uint8_t* pk48, const uint8_t* sig96, const
 }
 // same check, but the caller learns WHY an item failed, in the order the reference meets the errors: the sender key is decoded
 // first (BytesToBLSPublicKey, consensus/view_change_msg.go:159), then the signature (Sign.Deserialize, :168-179), then VerifyHash
-int hbls_verify_batch_status(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* status) {
-    if (int e = ensure_init()) return e;
-    if (k == 0) return 0;
-    if (!status) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+static int verify_batch_status_locked(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* status) {
     std::vector<uint8_t> flags(k);
     if (int e = verify_batch_locked(k, pk48, sig96, msgs, msg_len, status, flags.data())) return e;
     for (size_t j = 0; j < k; j++) {
@@ -1217,6 +1237,13 @@ int hbls_verify_batch_status(size_t k, const uint8_t* pk48, const uint8_t* sig96
         else status[j] = status[j] == 1 ? HBLS_VB_OK : HBLS_VB_BAD_SIG;
     }
     return 0;
+}
+int hbls_verify_batch_status(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* status) {
+    if (int e = ensure_init()) return e;
+    if (k == 0) return 0;
+    if (!status) return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return verify_batch_status_locked(k, pk48, sig96, msgs, msg_len, status);
 }
 
 // ------------------------------------------------------------------ persistent Mask / running vote aggregate (SURVEY 8f.2)
@@ -1296,10 +1323,7 @@ int hbls_ballot_box_create(hbls_ballot_box** out, const hbls_committee* c) {
     *out = b.release(); return 0;
 }
 void hbls_ballot_box_destroy(hbls_ballot_box* b) { if (!b) return; std::lock_guard<std::mutex> lk(g.mu); cudaDeviceSynchronize(); delete b; }
-int hbls_ballot_box_add_vote(hbls_ballot_box* b, const uint8_t* signer_bitmap, size_t blen, const uint8_t sig96[96]) {
-    if (int e = ensure_init()) return e;
-    if (!b || !signer_bitmap || blen != b->collected.size()) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+static int ballot_box_add_vote_locked(hbls_ballot_box* b, const uint8_t* signer_bitmap, size_t blen, const uint8_t sig96[96]) {
     const size_t n = b->c->n;
     for (size_t i = 0; i < n; i++)                                      // quorum.go:168-181: skip a ballot that shares a signer with a collected one
         if ((signer_bitmap[i >> 3] >> (i & 7)) & 1 && (b->collected[i >> 3] >> (i & 7)) & 1) return 1;
@@ -1315,10 +1339,13 @@ int hbls_ballot_box_add_vote(hbls_ballot_box* b, const uint8_t* signer_bitmap, s
     for (size_t i = 0; i < n; i++) if ((signer_bitmap[i >> 3] >> (i & 7)) & 1) b->collected[i >> 3] |= (uint8_t)(1u << (i & 7));
     return 0;
 }
-int hbls_ballot_box_aggregate(const hbls_ballot_box* b, uint8_t out_sig96[96], uint8_t* bitmap_out, size_t blen) {
+int hbls_ballot_box_add_vote(hbls_ballot_box* b, const uint8_t* signer_bitmap, size_t blen, const uint8_t sig96[96]) {
     if (int e = ensure_init()) return e;
-    if (!b || !out_sig96 || (bitmap_out && blen != b->collected.size())) return HBLS_ERR_ARG;
+    if (!b || !signer_bitmap || blen != b->collected.size()) return HBLS_ERR_ARG;
     std::lock_guard<std::mutex> lk(g.mu);
+    return ballot_box_add_vote_locked(b, signer_bitmap, blen, sig96);
+}
+static int ballot_box_aggregate_locked(const hbls_ballot_box* b, uint8_t out_sig96[96], uint8_t* bitmap_out, size_t blen) {
     Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};
     uint8_t* dout = ar.take<uint8_t>(96);
@@ -1328,16 +1355,19 @@ int hbls_ballot_box_aggregate(const hbls_ballot_box* b, uint8_t out_sig96[96], u
     if (bitmap_out) memcpy(bitmap_out, b->collected.data(), blen);
     return 0;
 }
+int hbls_ballot_box_aggregate(const hbls_ballot_box* b, uint8_t out_sig96[96], uint8_t* bitmap_out, size_t blen) {
+    if (int e = ensure_init()) return e;
+    if (!b || !out_sig96 || (bitmap_out && blen != b->collected.size())) return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return ballot_box_aggregate_locked(b, out_sig96, bitmap_out, blen);
+}
 
 // ------------------------------------------------------------------ ONE batch split over several GPUs (SURVEY 8e, BASELINE configs[3])
 struct PartialRecord { g2 S; fp2 f[6]; uint32_t n_items; uint32_t n_bad; };
 // the wire record is the first HBLS_PARTIAL_BYTES of the struct
 static_assert(offsetof(PartialRecord, n_bad) + sizeof(uint32_t) == HBLS_PARTIAL_BYTES && sizeof(PartialRecord) >= HBLS_PARTIAL_BYTES, "partial record layout");
-int hbls_rlc_partial(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t record[HBLS_PARTIAL_BYTES]) {
-    if (int e = ensure_init()) return e;
-    if (!record) return HBLS_ERR_ARG;
+static int rlc_partial_locked(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t record[HBLS_PARTIAL_BYTES]) {
     PartialRecord rec; memset(&rec, 0, sizeof rec);
-    std::lock_guard<std::mutex> lk(g.mu);
     const size_t kk = k ? k : 1;
     const unsigned W = (unsigned)(kk < (size_t)g.sm_count * 2 ? kk : (size_t)g.sm_count * 2);      // warps that multiply Miller values into partial products
     Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(kk) + kk * (48 + 96 + msg_len + 8) + (W + 2) * 6 * sizeof(fp2) + sizeof(g2) + 8192, &sc)) return e;
@@ -1372,13 +1402,14 @@ int hbls_rlc_partial(size_t k, const uint8_t* pk48, const uint8_t* sig96, const 
     memcpy(record, &rec, HBLS_PARTIAL_BYTES);
     return 0;
 }
-int hbls_rlc_fold(size_t n, const uint8_t* records) {
+int hbls_rlc_partial(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t record[HBLS_PARTIAL_BYTES]) {
     if (int e = ensure_init()) return e;
-    if (!records) return HBLS_ERR_ARG;
-    size_t items = 0, bad = 0;
-    for (size_t p = 0; p < n; p++) { PartialRecord r; memcpy(&r, records + p * HBLS_PARTIAL_BYTES, HBLS_PARTIAL_BYTES); items += r.n_items; bad += r.n_bad; }
-    if (bad || items == 0) return 0;                                  // an undecodable / identity item somewhere, or nothing to prove: callers verify exactly
+    if (!record) return HBLS_ERR_ARG;
     std::lock_guard<std::mutex> lk(g.mu);
+    return rlc_partial_locked(k, pk48, sig96, msgs, msg_len, record);
+}
+// the device part of hbls_rlc_fold (records that hold items and no undecodable one)
+static int rlc_fold_locked(size_t n, const uint8_t* records) {
     Scratch* sc; if (int e = reserve(g.stream, n * (sizeof(g2) + 6 * sizeof(fp2)) + sizeof(g2) + sizeof(g2a) + 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};
     g2* dS = ar.take<g2>(n); fp2* dparts = ar.take<fp2>(n * 6); g2* dsum = ar.take<g2>(1); g2a* dsg = ar.take<g2a>(1); uint8_t* dres = ar.take<uint8_t>(1);
@@ -1394,11 +1425,17 @@ int hbls_rlc_fold(size_t n, const uint8_t* records) {
     CK(cudaStreamSynchronize(g.stream));                              // hs / hf stay alive until the copies are done
     return res ? 1 : 0;
 }
-
-int hbls_sign_hash_batch(size_t k, const uint8_t* sk32, const uint8_t* msgs, size_t msg_len, uint8_t* sig96_out, uint8_t* ok) {
+int hbls_rlc_fold(size_t n, const uint8_t* records) {
     if (int e = ensure_init()) return e;
-    if (k == 0) return 0;
+    if (!records) return HBLS_ERR_ARG;
+    size_t items = 0, bad = 0;
+    for (size_t p = 0; p < n; p++) { PartialRecord r; memcpy(&r, records + p * HBLS_PARTIAL_BYTES, HBLS_PARTIAL_BYTES); items += r.n_items; bad += r.n_bad; }
+    if (bad || items == 0) return 0;                                  // an undecodable / identity item somewhere, or nothing to prove: callers verify exactly
     std::lock_guard<std::mutex> lk(g.mu);
+    return rlc_fold_locked(n, records);
+}
+
+static int sign_hash_batch_locked(size_t k, const uint8_t* sk32, const uint8_t* msgs, size_t msg_len, uint8_t* sig96_out, uint8_t* ok) {
     Scratch* sc; if (int e = reserve(g.stream, k * (32 + msg_len + sizeof(g2) + 96 + 1) + 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};
     uint8_t* dsk = ar.take<uint8_t>(k * 32); uint8_t* dmsg = ar.take<uint8_t>(k * msg_len + 1); g2* dpts = ar.take<g2>(k);
@@ -1412,10 +1449,13 @@ int hbls_sign_hash_batch(size_t k, const uint8_t* sk32, const uint8_t* msgs, siz
     CK(cudaStreamSynchronize(g.stream));
     return 0;
 }
-int hbls_get_public_key_batch(size_t k, const uint8_t* sk32, uint8_t* pk48_out) {
+int hbls_sign_hash_batch(size_t k, const uint8_t* sk32, const uint8_t* msgs, size_t msg_len, uint8_t* sig96_out, uint8_t* ok) {
     if (int e = ensure_init()) return e;
     if (k == 0) return 0;
     std::lock_guard<std::mutex> lk(g.mu);
+    return sign_hash_batch_locked(k, sk32, msgs, msg_len, sig96_out, ok);
+}
+static int get_public_key_batch_locked(size_t k, const uint8_t* sk32, uint8_t* pk48_out) {
     Scratch* sc; if (int e = reserve(g.stream, k * (32 + sizeof(g1) + 48) + 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};
     uint8_t* dsk = ar.take<uint8_t>(k * 32); g1* dpts = ar.take<g1>(k); uint8_t* dout = ar.take<uint8_t>(k * 48);
@@ -1426,11 +1466,14 @@ int hbls_get_public_key_batch(size_t k, const uint8_t* sk32, uint8_t* pk48_out) 
     CK(cudaStreamSynchronize(g.stream));
     return 0;
 }
-
-int hbls_fp_mul_batch(size_t n, const uint8_t* a48, const uint8_t* b48, uint8_t* out48) {
+int hbls_get_public_key_batch(size_t k, const uint8_t* sk32, uint8_t* pk48_out) {
     if (int e = ensure_init()) return e;
-    if (n == 0) return 0;
+    if (k == 0) return 0;
     std::lock_guard<std::mutex> lk(g.mu);
+    return get_public_key_batch_locked(k, sk32, pk48_out);
+}
+
+static int fp_mul_batch_locked(size_t n, const uint8_t* a48, const uint8_t* b48, uint8_t* out48) {
     Scratch* sc; if (int e = reserve(g.stream, n * 144 + 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};
     uint8_t* da = ar.take<uint8_t>(n * 48); uint8_t* db = ar.take<uint8_t>(n * 48); uint8_t* dout = ar.take<uint8_t>(n * 48);
@@ -1440,6 +1483,12 @@ int hbls_fp_mul_batch(size_t n, const uint8_t* a48, const uint8_t* b48, uint8_t*
     CK(cudaMemcpyAsync(out48, dout, n * 48, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
     return 0;
+}
+int hbls_fp_mul_batch(size_t n, const uint8_t* a48, const uint8_t* b48, uint8_t* out48) {
+    if (int e = ensure_init()) return e;
+    if (n == 0) return 0;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return fp_mul_batch_locked(n, a48, b48, out48);
 }
 
 void hbls_stage_timing_enable(int on) {
@@ -1457,9 +1506,7 @@ int hbls_stage_timing_get(float* ms_out, int max_stages) {
     if (max_stages >= 7) { float ms = 0; if (sc->ev7_set) cudaEventElapsedTime(&ms, sc->ev[5], sc->ev[7]); ms_out[6] = ms; n = 7; }
     return n;
 }
-int hbls_selftest_split(uint32_t iters) {
-    if (int e = ensure_init()) return e;
-    std::lock_guard<std::mutex> lk(g.mu);
+static int selftest_split_locked(uint32_t iters) {
     Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
     uint32_t* d = reinterpret_cast<uint32_t*>(sc->base);
     CK(cudaMemsetAsync(d, 0, 4, g.stream));
@@ -1468,6 +1515,11 @@ int hbls_selftest_split(uint32_t iters) {
     CK(cudaMemcpyAsync(&bad, d, 4, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
     return (int)bad;
+}
+int hbls_selftest_split(uint32_t iters) {
+    if (int e = ensure_init()) return e;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return selftest_split_locked(iters);
 }
 double hbls_probe_mac32_per_s(int iters, double* sm_clock_hz) {
     if (ensure_init()) return -1.0;
@@ -1491,3 +1543,5 @@ double hbls_probe_mac32_per_s(int iters, double* sm_clock_hz) {
 }
 
 }  // extern "C"
+
+#include "selftest.cuh"

@@ -38,6 +38,7 @@ extern "C" {
 #define HBLS_ERR_CUDA   (-100)      /* no device / CUDA runtime failure (message on stderr) */
 #define HBLS_ERR_ARG    (-2)        /* bad argument (e.g. bitmap length mismatch: mask.go:114-120) */
 #define HBLS_ERR_DECODE (-3)        /* an input failed to decode (not on curve / >= p / not in subgroup) */
+#define HBLS_ERR_SELF_TEST (-4)     /* the self-test run at initialisation (HBLS_SELF_TEST=1) failed: the library refuses all work */
 
 /* ------------------------------------------------------------------ Part 1: herumi bls.h shape (SWAP_G) */
 typedef struct { uint64_t d[4]; }  blsSecretKey;   /* 32 B: scalar < r, little-endian */
@@ -273,6 +274,24 @@ int hbls_stage_timing_get(float* ms_out, int max_stages);
  * pipe peak is sm_count * 4 schedulers * 8 MAC/clk * SM clock (bench.py uses the clock nvidia-smi reports under load and
  * reports the probe's share of it).  <0 on error */
 double hbls_probe_mac32_per_s(int iters, double* sm_clock_hz);
+
+/* Known-answer self-test of every kernel this library launches (except the roofline probe above), on a 16-key committee and a few
+ * hundred rounds at most, compared byte for byte with answers built into the library (csrc/selftest_kat.h, made by the CPU oracle).
+ * Organised as legs: bit i of failed_legs is leg i (names: hbls_self_test_leg_name).  Tuning paths a leg needs are forced for the leg
+ * and restored afterwards.  Threading: the self-test holds the library mutex for its whole duration, so every other call waits.
+ * It leaves the caller's state as it found it -- hbls_get_param values, the batch mode, stage timing and its recorded times,
+ * hbls_last_batch_info, the H(m) cache (entries and hbls_hash_cache_stats), hbls_coalesce_stats -- except that
+ * hbls_kernel_launch_count grows and the coefficient stream of the batched checks advances.
+ * With HBLS_SELF_TEST=1 in the environment, blsInit / hbls_init_device run it after initialising; when a leg fails they print the
+ * failing legs on stderr and return HBLS_ERR_SELF_TEST, and from then on every call fails (later init calls too, without a rerun).
+ * Returns 0 when every leg passes, the number of failed legs, or HBLS_ERR_CUDA on a runtime failure.  out (nullable). */
+typedef struct { uint64_t failed_legs; uint32_t legs; uint32_t kernels; float ms; } hbls_self_test_report;
+int hbls_self_test(hbls_self_test_report* out);
+/* name of leg `leg` into buf (NUL-terminated, truncated to cap): 0, or HBLS_ERR_ARG when there is no such leg */
+int hbls_self_test_leg_name(int leg, char* buf, size_t cap);
+/* the distinct kernels the last run launched, newline-separated, into buf (NUL-terminated, truncated to cap; buf nullable):
+ * returns the length of the whole list */
+int hbls_self_test_kernels(char* buf, size_t cap);
 
 #ifdef __cplusplus
 }
