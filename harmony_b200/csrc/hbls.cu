@@ -44,6 +44,8 @@ struct Ctx {
     int batch_mode = 1;                                     // 1: random-linear-combination groups + exact pass over failed groups, 0: exact per round
     // tuning (hbls_set_param)
     long long rlc_min = 12288, rlc_g = 0, tpsm = 384, tpsm_split = 512, tpsm_light = 1024, coop_max = 4096, overlap = 1, coop_wpsm = 14, hash_coop_max = 528, mask_sort = 1, hash_split = 2, tpsm_sw = 512, hash_fallback = 0, rlc_two_phase = 2, tpsm_lines = 512, tpsm_accum = 512, tpsm_cof = 512, tpsm_dec = 512, tpsm_scale = 384, tpsm_scale_g1 = 384, scale_split = 1, decode_split = 1, exact_two_phase = 1;
+    int* rlc_form = nullptr;                                // device: 1 = the last call that could use blocks had many failed groups (k_rlc_form)
+    long long rlc_block = 0;                                // blocks of HB_RLC_M groups (rlc_blocks): 0 automatic, 1 forced on, 2 forced off
     // coefficient stream: ChaCha20 keyed from /dev/urandom, block counter = call number
     uint32_t chacha_key[8] = {}; uint64_t rlc_calls = 0;
     // last batch
@@ -207,6 +209,15 @@ rlc_coeffs rlc_draw() {
     return co;
 }
 
+// blocks: one draw per (position inside a group, member of a block), 16 ChaCha20 blocks of the call's counter
+rlc_block_coeffs rlc_draw_block() {
+    rlc_block_coeffs cb; const uint64_t call = ++g.rlc_calls; uint32_t blk[16];
+    for (int i = 0; i < HB_RLC_GMAX * HB_RLC_M; i++) {
+        if ((i & 7) == 0) chacha20_block(g.chacha_key, call, blk, (uint32_t)(i >> 3) + 1);
+        cb.c[i / HB_RLC_M][i % HB_RLC_M] = ((uint64_t)blk[2 * (i & 7) + 1] << 32) | blk[2 * (i & 7)];
+    }
+    return cb;
+}
 // one independent draw per item (the single combined check of hbls_rlc_partial / hbls_rlc_fold)
 std::vector<uint64_t> rlc_draw_items(size_t k) {
     std::vector<uint64_t> c(k); const uint64_t call = ++g.rlc_calls; uint32_t blk[16];
@@ -241,13 +252,15 @@ size_t rlc_lines_bytes(size_t B) {
     const size_t list_bytes = g.exact_two_phase ? (size_t)HB_ML_STEPS * 3 * 2 * nlc * 2 * sizeof(fp) + B * sizeof(g2a) + 256 : 0;
     return (rlc_bytes > list_bytes ? rlc_bytes : list_bytes) + 256;
 }
+// blocks per call at most: S <= ceil(ng / HB_RLC_M) + 31
+size_t rlc_nblocks_max(size_t B) { return B / HB_RLC_G / HB_RLC_M + 32; }
 size_t verify_scratch_bytes(size_t B) {
-    return B * (sizeof(g2a) * 2 + sizeof(g1a) * 2 + sizeof(g1) + sizeof(g2) + 16 + 4 + 7) + HB_MASK_BINS * 4 + (B / HB_RLC_G + 1) * (sizeof(g2a) + 8) + 44 * 256
+    return B * (sizeof(g2a) * 2 + sizeof(g1a) * 2 + sizeof(g1) + sizeof(g2) + 16 + 4 + 7) + HB_MASK_BINS * 4 + (B / HB_RLC_G + 1) * (sizeof(g2a) + 8) + rlc_nblocks_max(B) * (sizeof(g2a) + 1) + 46 * 256
            + (B <= 8192 ? B * (12 * sizeof(fp2) + 3) + 1024 : 0)                // latency path: Miller values of (B, sigma) and (-apk, H(m))
            + rlc_lines_bytes(B);                                                 // two-kernel pairing: the line functions of one chunk
 }
 struct VerifyBufs { g2a* sig; g2a* hm; g1a* pkneg; g1* apk; uint8_t* ok_sig; uint8_t* ok_hm; uint8_t* ok_pk;
-                    g1a* pk_scaled; g2* S; uint8_t* bad; g2a* Sg; uint8_t* group_ok; uint32_t* fail_list; unsigned* counts;
+                    g1a* pk_scaled; g2* S; uint8_t* bad; g2a* Sg; uint8_t* group_ok; uint32_t* fail_list; unsigned* counts; g2a* Sb; uint8_t* block_ok;
                     fp2* f1; uint8_t* irr1; fp2* f2; uint8_t* irr2; uint8_t* ok_sub;
                     uint16_t* mask_cost; unsigned* mask_hist; uint32_t* mask_order; fp* lines; uint8_t* verdict; };
 VerifyBufs carve_verify(Arena& ar, size_t B) {
@@ -256,7 +269,8 @@ VerifyBufs carve_verify(Arena& ar, size_t B) {
     v.ok_sig = ar.take<uint8_t>(B); v.ok_hm = ar.take<uint8_t>(B); v.ok_pk = ar.take<uint8_t>(B);
     v.pk_scaled = ar.take<g1a>(B); v.S = ar.take<g2>(B); v.bad = ar.take<uint8_t>(B);
     v.Sg = ar.take<g2a>(B / HB_RLC_G + 1); v.group_ok = ar.take<uint8_t>(B / HB_RLC_G + 1);
-    v.fail_list = ar.take<uint32_t>(B); v.counts = ar.take<unsigned>(2);
+    v.fail_list = ar.take<uint32_t>(B); v.counts = ar.take<unsigned>(5);      // [0] [1] k_rlc_finish, [2] [3] form gates, [4] per-group check list
+    v.Sb = ar.take<g2a>(rlc_nblocks_max(B)); v.block_ok = ar.take<uint8_t>(rlc_nblocks_max(B));
     v.mask_cost = ar.take<uint16_t>(B); v.mask_hist = ar.take<unsigned>(HB_MASK_BINS); v.mask_order = ar.take<uint32_t>(B);
     v.verdict = ar.take<uint8_t>(B);
     v.lines = nullptr;
@@ -275,6 +289,15 @@ void fork_point(size_t B, Scratch* sc, cudaStream_t s) {
 // batched (random-linear-combination) form applies: default mode and a batch large enough
 static bool rlc_applies(size_t B) { return g.batch_mode == 1 && (long long)B >= g.rlc_min && B >= 2 * HB_RLC_GMAX; }
 static bool latency_path(size_t B) { return !rlc_applies(B) && (long long)B <= g.coop_max; }
+// blocks of HB_RLC_M groups share one final exponentiation and one generator pair (kernels.cuh: rlc_block_coeffs).  They need the
+// two-kernel pairing with every group in ONE chunk of the line buffer (a block must not span chunks); automatically from one whole
+// block on, rlc_block = 1 / 2 forces them on / off (wherever they can run at all)
+static bool rlc_blocks(size_t ng, bool two_phase) {
+    if (!two_phase || g.rlc_block == 2 || ng > rlc_chunk_groups()) return false;
+    return g.rlc_block == 1 || ng >= HB_RLC_M;
+}
+// the groups' Miller values of the block form: 6 Fp2 per group, behind the G round pairs' lines (the buffer holds G + 1 pairs)
+static fp2* rlc_fm(const VerifyBufs& v, size_t G, size_t ng) { return reinterpret_cast<fp2*>(v.lines + (size_t)HB_ML_STEPS * 3 * G * ng * 2); }
 // exact checks of batches beyond the warp-per-round range run as line kernel + accumulator kernel too (twice the lane pairs in the
 // first one; the second no longer carries the running points)
 static bool exact_two_phase(size_t B) { return g.rlc_two_phase >= 2 && g.exact_two_phase && !rlc_applies(B) && (long long)B > g.coop_max; }
@@ -348,21 +371,29 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
     STAGE_EV(4, sc, s);
     hbls_batch_info& bi = g.info;
     bi = hbls_batch_info{}; bi.rounds = B; bi.mode = rlc ? 1 : 0;
-    cudaMemsetAsync(v.counts, 0, 2 * sizeof(unsigned), s);
+    cudaMemsetAsync(v.counts, 0, 5 * sizeof(unsigned), s);
     if (rlc) {
         // batched form (north-star "batched Miller loop + shared final exponentiation"): strided groups of G rounds; G = 8 once
         // that still gives every SM a full CTA of lane pairs (fewer Miller-loop pairs and final exponentiations per round), else 4
         const size_t G = rlc_group_size(B);
         const size_t ng = B / G, nr = ng * G, tail = B - nr;
         const rlc_coeffs co = rlc_draw();
-        if (g.scale_split && HB_BATCH_INV) {
-            LAUNCH(k_rlc_scale_g1, capped_blocks(nr, g.tpsm_scale_g1, TPB), TPB, s, nr, ng, v.apk, co, v.pk_scaled);
-            LAUNCH(k_rlc_scale_g2, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad);
-        } else
-        LAUNCH(k_rlc_scale, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, (const uint64_t*)nullptr, v.pk_scaled, v.S, v.bad);
         const bool full = 2 * ng >= (size_t)g.sm_count * HB_TPB_SPLIT;
         const unsigned pb = full ? split_blocks(2 * ng) : blocks_for(2 * ng, 64), pt = full ? HB_TPB_SPLIT : 64;
         const bool two_phase = g.rlc_two_phase && v.lines != nullptr && (full || g.rlc_two_phase >= 2);
+        // blocks of HB_RLC_M groups: group g is member g / S of block g mod S; coefficients per (position, member)
+        const bool blocks = rlc_blocks(ng, two_phase);
+        const size_t S = blocks ? (((ng + HB_RLC_M - 1) / HB_RLC_M + 31) & ~(size_t)31) : 0;
+        const rlc_block_coeffs cb = blocks ? rlc_draw_block() : rlc_block_coeffs{};
+        // blocks possible: the device picks the form from how the last such call ended (k_rlc_form); counts[2] / counts[3] gate the
+        // group form's / block form's kernels, the scaling kernels take the matching coefficients
+        const unsigned* blk_gate = blocks ? v.counts + 3 : nullptr;
+        if (blocks) LAUNCH(k_rlc_form, 1, 32, s, ng, g.rlc_block == 1 ? 1 : 0, (const int*)g.rlc_form, v.counts + 2);
+        if (g.scale_split && HB_BATCH_INV) {
+            LAUNCH(k_rlc_scale_g1, capped_blocks(nr, g.tpsm_scale_g1, TPB), TPB, s, nr, ng, v.apk, co, v.pk_scaled, S, cb, blk_gate);
+            LAUNCH(k_rlc_scale_g2, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+        } else
+        LAUNCH(k_rlc_scale, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, (const uint64_t*)nullptr, v.pk_scaled, v.S, v.bad, S, cb, blk_gate);
         if (G == 8) LAUNCH(k_rlc_group_sum<8>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
         else LAUNCH(k_rlc_group_sum<4>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
         STAGE_EV(5, sc, s);
@@ -376,11 +407,32 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
                 const unsigned lt = full ? cta(g.tpsm_lines) : 64, at = full ? cta(g.tpsm_accum) : 64;
                 const unsigned lb = full ? capped_blocks(2 * (G + 1) * ngc, lt, lt) : blocks_for(2 * (G + 1) * ngc, 64);
                 const unsigned ab = full ? capped_blocks(2 * ngc, at, at) : blocks_for(2 * ngc, 64);
-                if (G == 8) LAUNCH(k_rlc_lines_split<8>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.Sg, v.lines);
-                else LAUNCH(k_rlc_lines_split<4>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.Sg, v.lines);
+                // blocks possible (one chunk): both forms are launched and the device gates (k_rlc_form) let exactly one of them run
+                const unsigned* gate_groups = blocks ? v.counts + 2 : nullptr;
+                const unsigned* gate_blocks = v.counts + 3;
+                if (G == 8) LAUNCH(k_rlc_lines_split<8>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.Sg, v.lines, gate_groups);
+                else LAUNCH(k_rlc_lines_split<4>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.Sg, v.lines, gate_groups);
+                if (blocks && G == 8) LAUNCH(k_rlc_lines_blk<8>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.lines, gate_blocks);
+                else if (blocks) LAUNCH(k_rlc_lines_blk<4>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.lines, gate_blocks);
                 if (g0 == 0) { STAGE_EV(7, sc, s); sc->ev7_set = g.stage_timing && sc->ev_ok; }       // line kernel | accumulator kernel (first chunk)
-                if (G == 8) LAUNCH(k_rlc_accum_split<8>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok);
-                else LAUNCH(k_rlc_accum_split<4>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok);
+                if (G == 8) LAUNCH(k_rlc_accum_split<8>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, gate_groups);
+                else LAUNCH(k_rlc_accum_split<4>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, gate_groups);
+                if (blocks && G == 8) LAUNCH(k_rlc_accum_blk<8>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, rlc_fm(v, G, ng), gate_blocks);
+                else if (blocks) LAUNCH(k_rlc_accum_blk<4>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, rlc_fm(v, G, ng), gate_blocks);
+            }
+            if (blocks) {
+                // one final exponentiation and one generator pair per block (warp per block), then the groups of the failed blocks
+                // alone: FE( their Miller value * Miller(B, Sg) ) == 1, a lane pair each, the list spread evenly over the lock-stepped
+                // CTAs.  group_ok then holds every group's own verdict, as without blocks.
+                fp2* fm = rlc_fm(v, G, ng);
+                const unsigned cb_grid = full ? split_blocks(2 * ng) : blocks_for(2 * ng, 64), cb_tpb = full ? HB_TPB_SPLIT : 64;
+                const unsigned* gate = v.counts + 3;
+                LAUNCH(k_rlc_block_sum, heavy_blocks(S), TPB, s, S, ng, (const g2a*)v.Sg, v.Sb, gate);
+                const size_t coop_cap = (size_t)g.sm_count * (size_t)(g.coop_wpsm > 0 ? g.coop_wpsm : 1);
+                LAUNCH(k_rlc_block_coop, (unsigned)(S < coop_cap ? S : coop_cap), 32, s, S, ng, (const fp2*)fm, (const g2a*)v.Sb, (const uint8_t*)v.group_ok, v.block_ok, gate);
+                LAUNCH(k_rlc_block_list, blocks_for(ng, 256), 256, s, ng, S, (const uint8_t*)v.block_ok, v.group_ok, v.fail_list, v.counts + 4, gate);
+                LAUNCH(k_rlc_group_check_list, cb_grid, cb_tpb, s, (const unsigned*)v.counts + 4, (const uint32_t*)v.fail_list, (const fp2*)fm,
+                       (const g2a*)v.Sg, v.group_ok);
             }
         } else if (G == 8)
             LAUNCH_SMEM(k_rlc_pairing_split<8>, pb, pt, HB_SMEM_F ? pt * HB_SMEM_F_WORDS * 4 : 0, s, ng, v.pk_scaled, v.hm, v.Sg, v.bad, v.group_ok);
@@ -389,6 +441,7 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
         // exact pass over the rounds of failed groups only (compacted on the device; the launches are sized for the worst case and
         // return at once when the list is short or empty)
         LAUNCH(k_rlc_finish, blocks_for(nr, 256), 256, s, nr, ng, v.group_ok, d_results, v.fail_list, v.counts);
+        if (blocks) LAUNCH(k_rlc_form_update, 1, 32, s, ng, (const unsigned*)v.counts, g.rlc_form);     // the next call's form
         LAUNCH(k_g1_normalize_list, heavy_blocks(nr), TPB, s, v.counts, v.fail_list, v.apk, v.pkneg, 1);
         if (two_phase && g.exact_two_phase) {
             // the listed rounds, gathered into contiguous arrays, through the line / accumulator kernels as "groups" of one round; the
@@ -852,11 +905,13 @@ int hbls_init_device(int device) {
     CK(cudaFuncSetAttribute(k_mask_aggregate_serial, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_mask_aggregate, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaMalloc(&g.hm_slots, Ctx::HM_N * sizeof(g2a))); CK(cudaMalloc(&g.hm_ok, Ctx::HM_N));
+    CK(cudaMalloc(&g.rlc_form, sizeof(int))); CK(cudaMemset(g.rlc_form, 0, sizeof(int)));
     for (int i = 0; i < Ctx::HM_N; i++) {
         CK(cudaEventCreateWithFlags(&g.hm[i].filled, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&g.hm[i].read_done, cudaEventDisableTiming));
     }
     g.hm_cache = envll("HBLS_HM_CACHE", 1); g.mask_sort = envll("HBLS_MASK_SORT", 1); g.hash_coop_max = envll("HBLS_HASH_COOP_MAX", 4ll * g.sm_count);     // one warp per message while every scheduler gets one
     g.rlc_two_phase = envll("HBLS_RLC_2P", 2); g.tpsm_lines = envll("HBLS_TPSM_LINES", 512); g.tpsm_accum = envll("HBLS_TPSM_ACCUM", 512); g.tpsm_cof = envll("HBLS_TPSM_COF", 512); g.tpsm_dec = envll("HBLS_TPSM_DEC", 512); g.tpsm_scale = envll("HBLS_TPSM_SCALE", 384); g.tpsm_scale_g1 = envll("HBLS_TPSM_SCALE_G1", 384); g.scale_split = envll("HBLS_SCALE_SPLIT", 1); g.decode_split = envll("HBLS_DECODE_SPLIT", 1); g.exact_two_phase = envll("HBLS_EXACT_2P", 1);
+    g.rlc_block = envll("HBLS_RLC_BLOCK", 0);
     g.hash_split = envll("HBLS_HASH_SPLIT", 2); g.tpsm_sw = envll("HBLS_TPSM_SW", 512);
     CK(cudaFuncSetAttribute(k_hash_sw, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_hash_cofactor, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
@@ -882,7 +937,7 @@ const ParamDef PARAMS[] = {
     {"overlap", &Ctx::overlap}, {"coop_wpsm", &Ctx::coop_wpsm}, {"hm_cache", &Ctx::hm_cache}, {"hash_coop_max", &Ctx::hash_coop_max}, {"mask_sort", &Ctx::mask_sort}, {"hash_split", &Ctx::hash_split},
     {"hash_fallback", &Ctx::hash_fallback}, {"rlc_two_phase", &Ctx::rlc_two_phase}, {"tpsm_cof", &Ctx::tpsm_cof}, {"tpsm_dec", &Ctx::tpsm_dec}, {"tpsm_scale", &Ctx::tpsm_scale}, {"tpsm_scale_g1", &Ctx::tpsm_scale_g1},
     {"scale_split", &Ctx::scale_split}, {"decode_split", &Ctx::decode_split}, {"exact_two_phase", &Ctx::exact_two_phase}, {"tpsm_lines", &Ctx::tpsm_lines}, {"tpsm_accum", &Ctx::tpsm_accum}, {"tpsm_sw", &Ctx::tpsm_sw},
-    {"selftest_flip", &Ctx::selftest_flip}};
+    {"rlc_block", &Ctx::rlc_block}, {"selftest_flip", &Ctx::selftest_flip}};
 static long long* param_slot(const char* name) {
     if (!name) return nullptr;
     for (const ParamDef& p : PARAMS) if (!strcmp(name, p.name)) return &(g.*p.slot);
@@ -893,6 +948,7 @@ int hbls_set_param(const char* name, long long value) {
     long long* p = param_slot(name);
     if (!p || value < 0) return HBLS_ERR_ARG;
     if (p == &g.rlc_g && value != 0 && value != 4 && value != 8) return HBLS_ERR_ARG;
+    if (p == &g.rlc_block && value > 2) return HBLS_ERR_ARG;
     *p = value; return 0;
 }
 long long hbls_get_param(const char* name) { std::lock_guard<std::mutex> lk(g.mu); long long* p = param_slot(name); return p ? *p : -1; }

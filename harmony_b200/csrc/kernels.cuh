@@ -745,14 +745,31 @@ __global__ void __launch_bounds__(32) k_pairing_coop2(size_t B, const fp2* f1, c
 // share one scalar and the double-and-add ladders run without divergence.  Sharing c[k] across groups is sound: every group's
 // test passes wrongly with probability <= 2^-63 over the draw, whatever the (non-adaptive) input.
 struct rlc_coeffs { uint64_t c[HB_RLC_GMAX]; };
+// Blocks (hbls.cu rlc_blocks): HB_RLC_M groups share ONE final exponentiation and ONE generator pair.  Group g is member m = g / S of
+// block b = g mod S, S = ceil(ng / HB_RLC_M) rounded up to a multiple of 32, so the 32 consecutive groups of a warp of the scaling
+// kernels share (k, m) and their ladders stay warp-uniform.  Equal coefficients would no longer do: two bad rounds at the same
+// position of two groups of one block (sigma_a + D, sigma_b - D) would cancel in the block's product.  So every (position, member)
+// gets its own draw and only (0, 0) keeps 1.
+#define HB_RLC_M 16
+struct rlc_block_coeffs { uint64_t c[HB_RLC_GMAX][HB_RLC_M]; };
+// coefficient of round j = k ng + g: per position (S = 0: every group checked on its own), or per (position, block member)
+HB_DEV uint64_t rlc_coeff(const rlc_coeffs& co, size_t j, size_t ng, size_t S, const rlc_block_coeffs& cb) {
+    const size_t k = j / ng;
+    if (!S) return k ? co.c[k] : 1ull;
+    const size_t m = (j - k * ng) / S;
+    return (k | m) ? cb.c[k][m] : 1ull;
+}
 // per round: P_j = -r_j apk_j (affine), S_j = r_j sigma_j (Jacobian), bad_j
 #ifndef HB_SCALE_MINBLOCKS
 #define HB_SCALE_MINBLOCKS 1
 #endif
 __global__ void __launch_bounds__(64, HB_SCALE_MINBLOCKS) k_rlc_scale(size_t B, size_t ng, const g1* apk, const g2a* sig, const g2a* hm, const uint8_t* ok_sig, const uint8_t* ok_hm,
-                            const uint8_t* ok_pk, rlc_coeffs co, const uint64_t* per_item, g1a* pk_scaled_neg, g2* S, uint8_t* bad) {
+                            const uint8_t* ok_pk, rlc_coeffs co, const uint64_t* per_item, g1a* pk_scaled_neg, g2* S, uint8_t* bad,
+                            size_t blk_stride = 0, rlc_block_coeffs cb = {}, const unsigned* blk_gate = nullptr) {
+  if (blk_gate && *blk_gate == 0) blk_stride = 0;        // the device chose the group form (k_rlc_form): per-position coefficients
   // per_item (nullable): one independent coefficient per round -- needed when ALL rounds enter one combined check (the split of a
-  // single batch over several GPUs, k_rlc_partial_coop); the grouped form shares co.c[position in group] across groups
+  // single batch over several GPUs, k_rlc_partial_coop); the grouped form shares co.c[position in group] across groups, the block
+  // form (blk_stride = S != 0) cb.c[position][member]
 #if HB_BATCH_INV
   for (size_t j0 = HB_TID; j0 < B; j0 += (size_t)HB_BATCH_K * HB_STRIDE) {
     g1 ra[HB_BATCH_K]; fp z[HB_BATCH_K]; bool skip[HB_BATCH_K];
@@ -764,7 +781,7 @@ __global__ void __launch_bounds__(64, HB_SCALE_MINBLOCKS) k_rlc_scale(size_t B, 
         // rounds of a warp share their position).  Sound: a group holding a bad round passes only if prod_j delta_j^{s_j} = 1 with
         // some delta_j != 1; if that j is 0 alone the product is delta_0 != 1, otherwise one of the random s_j (j >= 1) must hit
         // the single value mod r that cancels the rest -- probability <= 2^-63, as before.
-        const uint64_t r = per_item ? per_item[j] : (j < ng ? 1ull : co.c[j / ng]);
+        const uint64_t r = per_item ? per_item[j] : rlc_coeff(co, j, ng, blk_stride, cb);
         g1 a = apk[j]; g2a sg = sig[j]; g2a h = hm[j];
         const bool b = !ok_sig[j] || !ok_hm[j] || (ok_pk && !ok_pk[j]) || pt_is_inf(a) || aff_is_inf(sg) || aff_is_inf(h);
         g2 rs;
@@ -784,7 +801,7 @@ __global__ void __launch_bounds__(64, HB_SCALE_MINBLOCKS) k_rlc_scale(size_t B, 
   }
 #else
   for (size_t j = HB_TID; j < B; j += HB_STRIDE) {
-    const uint64_t r = per_item ? per_item[j] : (j < ng ? 1ull : co.c[j / ng]);
+    const uint64_t r = per_item ? per_item[j] : rlc_coeff(co, j, ng, blk_stride, cb);
     g1 a = apk[j]; g2a sg = sig[j]; g2a h = hm[j];
     const bool b = !ok_sig[j] || !ok_hm[j] || (ok_pk && !ok_pk[j]) || pt_is_inf(a) || aff_is_inf(sg) || aff_is_inf(h);
     g1 ra; g2 rs;
@@ -796,7 +813,9 @@ __global__ void __launch_bounds__(64, HB_SCALE_MINBLOCKS) k_rlc_scale(size_t B, 
 }
 // the same stage as two kernels, one ladder each (hbls.cu "scale_split"): the G1 ladder (+ shared-inversion affine conversion) and the
 // G2 ladder are different code over different fields, and one kernel holding both stalls on instruction fetch
-__global__ void k_rlc_scale_g1(size_t B, size_t ng, const g1* apk, rlc_coeffs co, g1a* pk_scaled_neg) {
+__global__ void k_rlc_scale_g1(size_t B, size_t ng, const g1* apk, rlc_coeffs co, g1a* pk_scaled_neg, size_t blk_stride = 0, rlc_block_coeffs cb = {},
+                               const unsigned* blk_gate = nullptr) {
+  if (blk_gate && *blk_gate == 0) blk_stride = 0;
   for (size_t j0 = HB_TID; j0 < B; j0 += (size_t)HB_BATCH_K * HB_STRIDE) {
     g1 ra[HB_BATCH_K]; fp z[HB_BATCH_K]; bool skip[HB_BATCH_K];
     for (int k = 0; k < HB_BATCH_K; k++) {
@@ -804,7 +823,8 @@ __global__ void k_rlc_scale_g1(size_t B, size_t ng, const g1* apk, rlc_coeffs co
         skip[k] = true;
         if (j >= B) continue;
         const g1 a = apk[j];
-        if (j < ng) ra[k] = a; else rlc_scale_g1(ra[k], a, co.c[j / ng]);
+        const uint64_t r = rlc_coeff(co, j, ng, blk_stride, cb);
+        if (r == 1ull) ra[k] = a; else rlc_scale_g1(ra[k], a, r);
         skip[k] = pt_is_inf(ra[k]);
         if (!skip[k]) z[k] = ra[k].z;
     }
@@ -822,12 +842,15 @@ __global__ void k_rlc_scale_g1(size_t B, size_t ng, const g1* apk, rlc_coeffs co
 #define HB_SCALE_G2_MINBLOCKS 1
 #endif
 __global__ void __launch_bounds__(64, HB_SCALE_G2_MINBLOCKS) k_rlc_scale_g2(size_t B, size_t ng, const g1* apk, const g2a* sig, const g2a* hm, const uint8_t* ok_sig, const uint8_t* ok_hm,
-                               const uint8_t* ok_pk, rlc_coeffs co, g2* S, uint8_t* bad) {
+                               const uint8_t* ok_pk, rlc_coeffs co, g2* S, uint8_t* bad, size_t blk_stride = 0, rlc_block_coeffs cb = {},
+                               const unsigned* blk_gate = nullptr) {
+  if (blk_gate && *blk_gate == 0) blk_stride = 0;
   for (size_t j = HB_TID; j < B; j += HB_STRIDE) {
     const g2a sg = sig[j];
     const bool b = !ok_sig[j] || !ok_hm[j] || (ok_pk && !ok_pk[j]) || fp_is_zero(apk[j].z) || aff_is_inf(sg) || aff_is_inf(hm[j]);
     g2 rs;
-    if (j < ng) pt_from_aff(rs, sg); else rlc_scale_g2(rs, sg, co.c[j / ng]);
+    const uint64_t r = rlc_coeff(co, j, ng, blk_stride, cb);
+    if (r == 1ull) pt_from_aff(rs, sg); else rlc_scale_g2(rs, sg, r);
     S[j] = rs; bad[j] = b ? 1 : 0;
   }
 }
@@ -908,13 +931,15 @@ HB_DEV void line_load(fp& v, const fp* src) {
     v.l[0] = a.x; v.l[1] = a.y; v.l[2] = a.z; v.l[3] = a.w; v.l[4] = b.x; v.l[5] = b.y; v.l[6] = b.z; v.l[7] = b.w; v.l[8] = c.x; v.l[9] = c.y; v.l[10] = c.z; v.l[11] = c.w;
 #endif
 }
-template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_lines_split(size_t ngtot, size_t g0, size_t ngroups, const g1a* pk_scaled_neg, const g2a* hm,
-                                 const g2a* Sg, fp* lines, const unsigned* count = nullptr) {
+// BLK (blocks, hbls.cu rlc_blocks): only the G round pairs; the block check adds ONE pair (B, sum of the block's Sg).  A compile-time
+// choice, so the group form's kernels compile as they did without blocks.
+template <int G, bool BLK> HB_DEV void rlc_lines_body(size_t ngtot, size_t g0, size_t ngroups, const g1a* pk_scaled_neg, const g2a* hm,
+                                                     const g2a* Sg, fp* lines, const unsigned* count) {
     // groups g0 .. g0 + ngroups - 1 of ngtot (a chunk: the line buffer is sized for hbls.cu rlc_chunk_groups()); round of (k, g) = k * ngtot + g
-    // count (nullable): the number of groups is only known on the device (compacted list of the failed groups' rounds)
+    // count (nullable): the number of groups is only known on the device (compacted list of the failed groups' rounds; 0: nothing to do)
     if (count) { const size_t n = *count; if (g0 >= n) return; ngtot = n; ngroups = n - g0 < ngroups ? n - g0 : ngroups; }
     const int role = threadIdx.x & 1;
-    const size_t ppg = HB_STRIDE >> 1, npairs = (size_t)(G + 1) * ngroups;
+    const size_t ppg = HB_STRIDE >> 1, npairs = (size_t)(BLK ? G : G + 1) * ngroups;
     for (size_t it = 0; ; it++) {
         const size_t warp_first = it * ppg + ((HB_TID & ~(size_t)31) >> 1);
         if (warp_first >= npairs) break;
@@ -922,7 +947,7 @@ template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SP
         const bool valid = p < npairs;
         const size_t pp = valid ? p : npairs - 1, k = pp / ngroups, g = pp - k * ngroups;
         g1a P; const fp* q4;
-        if (k < (size_t)G) { P = pk_scaled_neg[k * ngtot + g0 + g]; q4 = reinterpret_cast<const fp*>(&hm[k * ngtot + g0 + g]); }
+        if (BLK || k < (size_t)G) { P = pk_scaled_neg[k * ngtot + g0 + g]; q4 = reinterpret_cast<const fp*>(&hm[k * ngtot + g0 + g]); }
         else { fp_set(P.x, K_G1_X); fp_set(P.y, K_G1_Y); q4 = reinterpret_cast<const fp*>(&Sg[g0 + g]); }
         fp2h qx, qy; qx.c = q4[role]; qy.c = q4[2 + role];
         g2proj_t<fp2h> T; T.x = qx; T.y = qy; fp2_one(T.z);
@@ -944,10 +969,22 @@ template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SP
         }
     }
 }
-template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_accum_split(size_t ngtot, size_t g0, size_t ngroups, const fp* lines, const uint8_t* bad, uint8_t* group_ok, const unsigned* count = nullptr) {
+template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_lines_split(size_t ngtot, size_t g0, size_t ngroups, const g1a* pk_scaled_neg, const g2a* hm,
+                                 const g2a* Sg, fp* lines, const unsigned* count = nullptr) {
+    rlc_lines_body<G, false>(ngtot, g0, ngroups, pk_scaled_neg, hm, Sg, lines, count);
+}
+template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_lines_blk(size_t ngtot, size_t g0, size_t ngroups, const g1a* pk_scaled_neg, const g2a* hm,
+                                 fp* lines, const unsigned* count = nullptr) {
+    rlc_lines_body<G, true>(ngtot, g0, ngroups, pk_scaled_neg, hm, nullptr, lines, count);
+}
+// BLK: the G round pairs only; the group's Miller value goes to fm (6 Fp2 per group, tower order) and group_ok gets "no bad round" --
+// the final exponentiation is the block check's (k_rlc_block_coop), or that of the per-group check (k_rlc_group_check_list)
+template <int G, bool BLK> HB_DEV void rlc_accum_body(size_t ngtot, size_t g0, size_t ngroups, const fp* lines, const uint8_t* bad, uint8_t* group_ok,
+                                                     const unsigned* count, fp2* fm) {
     if (count) { const size_t n = *count; if (g0 >= n) return; ngtot = n; ngroups = n - g0 < ngroups ? n - g0 : ngroups; }
     const int role = threadIdx.x & 1;
-    const size_t ppg = HB_STRIDE >> 1, npairs = (size_t)(G + 1) * ngroups;
+    constexpr int klast = BLK ? G - 1 : G;                              // last pair of a step: the generator pair, unless blocks
+    const size_t ppg = HB_STRIDE >> 1, npairs = (size_t)(klast + 1) * ngroups;
     for (size_t it = 0; ; it++) {
         const size_t warp_first = it * ppg + ((HB_TID & ~(size_t)31) >> 1);
         if (warp_first >= ngroups) break;
@@ -968,11 +1005,11 @@ template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SP
         auto mul_lines = [&](size_t step) {
             const fp* base = lines + ((step * 3) * npairs + gg) * 2 + role;
 #pragma unroll 1
-            for (int k = 0; k <= G; k += HB_LINE_PAIRS ? 2 : 1) {
+            for (int k = 0; k <= klast; k += HB_LINE_PAIRS ? 2 : 1) {
                 if (HB_ACCUM_SYNC > 0 && G > 4 && (k % (HB_ACCUM_SYNC > 0 ? HB_ACCUM_SYNC : 1)) == 0 && k) hb_lockstep<fp2h>();
                 const fp* o = base + (size_t)k * ngroups * 2;
                 fp2h l0, l2, l3; line_load(l0.c, o); line_load(l2.c, o + 2 * npairs); line_load(l3.c, o + 4 * npairs);
-                if (HB_LINE_PAIRS && k + 1 <= G) {
+                if (HB_LINE_PAIRS && k + 1 <= klast) {
                     const fp* o2 = o + ngroups * 2;
                     fp2h n0, n2, n3; line_load(n0.c, o2); line_load(n2.c, o2 + 2 * npairs); line_load(n3.c, o2 + 4 * npairs);
                     fp12_mul_by_two_lines(m, m, l0, l2, l3, n0, n2, n3);
@@ -986,10 +1023,134 @@ template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SP
             mul_lines(st++);
             if ((K_Z_ABS >> i) & 1) mul_lines(st++);
         }
+        if (BLK) {
+            if (valid) {
+                fp* o = reinterpret_cast<fp*>(fm + 6 * (g0 + g)) + role;
+                const fp2h* mc = reinterpret_cast<const fp2h*>(&m);
+                for (int t = 0; t < 6; t++) o[2 * t] = mc[t].c;
+                if (role == 0) group_ok[g0 + g] = anybad ? 0 : 1;
+            }
+            continue;
+        }
         final_exp(m, m);
         const bool one = fp12_is_one(m);
         if (valid && role == 0) group_ok[g0 + g] = (one && !anybad) ? 1 : 0;
     }
+}
+template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_accum_split(size_t ngtot, size_t g0, size_t ngroups, const fp* lines, const uint8_t* bad, uint8_t* group_ok,
+                                 const unsigned* count = nullptr) {
+    rlc_accum_body<G, false>(ngtot, g0, ngroups, lines, bad, group_ok, count, nullptr);
+}
+template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_accum_blk(size_t ngtot, size_t g0, size_t ngroups, const fp* lines, const uint8_t* bad, uint8_t* group_ok,
+                                 fp2* fm, const unsigned* count = nullptr) {
+    rlc_accum_body<G, true>(ngtot, g0, ngroups, lines, bad, group_ok, count, fm);
+}
+// ---- blocks of HB_RLC_M groups: one final exponentiation and one generator pair per block (hbls.cu rlc_blocks).
+// Per block b: Sb = sum of the Sg of its members (groups b, b + S, ...), affine
+// gate (nullable, every block kernel): the block form runs only while *gate != 0 (hbls.cu: k_rlc_form picks the form on the device)
+__global__ void k_rlc_block_sum(size_t S, size_t ng, const g2a* Sg, g2a* Sb, const unsigned* gate = nullptr) {
+  if (gate && *gate == 0) return;
+  for (size_t b = HB_TID; b < S; b += HB_STRIDE) {
+    g2 acc; pt_set_inf(acc);
+    for (size_t g = b; g < ng; g += S) { const g2a q = Sg[g]; pt_add_mixed(acc, acc, q); }
+    g2a a; pt_to_aff(a, acc); Sb[b] = a;
+  }
+}
+// the block check, ONE WARP per block (vm.cuh): FE( prod_m fm[member m] * Miller(B, Sb) ) == 1 and no member holds a bad round
+// (group_ok = "no bad round" from k_rlc_accum_split).  An identity Sb proves nothing: the block fails and its groups are checked alone.
+__global__ void __launch_bounds__(32) k_rlc_block_coop(size_t S, size_t ng, const fp2* fm, const g2a* Sb, const uint8_t* group_ok, uint8_t* block_ok,
+                                                       const unsigned* gate = nullptr) {
+    if (gate && *gate == 0) return;
+    __shared__ uint32_t slots[VM_SMEM_WORDS];
+    const int lane = threadIdx.x & 31;
+    vm_load_consts(slots);
+    for (size_t b = blockIdx.x; b < S; b += gridDim.x) {
+        bool clean = true;
+        for (size_t g = b; g < ng; g += S) clean &= group_ok[g] != 0;
+        if (!clean) { if (lane == 0) block_ok[b] = 0; __syncwarp(); continue; }      // warp-uniform
+        vm_run(VM_P_A_ONE, slots);
+        for (size_t g = b; g < ng; g += S) {
+            if (lane < 12) vm_st(slots, VM_R_F0 + (lane >> 1), lane & 1, reinterpret_cast<const fp*>(&fm[6 * g + (lane >> 1)])[lane & 1].l);
+            __syncwarp();
+            vm_run(VM_P_AMULF, slots);
+        }
+        bool zero = true;
+        if (lane < 4) {
+            fp2 v; fp2_zero(v);
+            if (lane == 0) fp_set(v.a, K_G1_X); else if (lane == 1) fp_set(v.a, K_G1_Y); else if (lane == 2) v = Sb[b].x; else v = Sb[b].y;
+            vm_set_fp2(slots, VM_R_P2X + lane, v);
+            zero = fp_is_zero(v.a) & fp_is_zero(v.b);
+        }
+        const unsigned zmask = __ballot_sync(0xffffffffu, zero);
+        bool one = false;
+        if ((zmask & 0xc) != 0xc) {
+            vm_run(VM_P_ML1_INIT, slots);
+            for (int i = 62; i >= 0; i--) {
+                vm_run(VM_P_ML1_DBL, slots);
+                if ((K_Z_ABS >> i) & 1) vm_run(VM_P_ML1_ADD, slots);
+            }
+            vm_run(VM_P_FMULA, slots);
+            one = vm_final_exp_is_one(slots);
+        }
+        if (lane == 0) block_ok[b] = one ? 1 : 0;
+        __syncwarp();
+    }
+}
+// groups of the blocks that failed: compacted into list (count on the device) for k_rlc_group_check_list.  A group of a proven block
+// keeps group_ok = 1; a group holding a bad round keeps 0 and needs no check of its own.
+__global__ void k_rlc_block_list(size_t ng, size_t S, const uint8_t* block_ok, uint8_t* group_ok, uint32_t* list, unsigned* count,
+                                 const unsigned* gate = nullptr) {
+    const size_t g = HB_TID; if (g >= ng || (gate && *gate == 0)) return;
+    if (block_ok[g % S] || !group_ok[g]) return;
+    group_ok[g] = 0;
+    list[atomicAdd(count, 1u)] = (uint32_t)g;
+}
+// lane pair per listed group: group_ok = FE( fm[g] * Miller(B, Sg[g]) ) == 1 -- the per-group check of k_rlc_accum_split without blocks
+__global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_group_check_list(const unsigned* count, const uint32_t* list, const fp2* fm,
+                                                                                         const g2a* Sg, uint8_t* group_ok) {
+    const size_t n = *count;
+    if (n == 0) return;
+    const int role = threadIdx.x & 1;
+    // lane pair q of CTA c takes item q * gridDim.x + c: a list shorter than the grid still gives every CTA (one per SM) its share,
+    // in its first warps, and the rest of the CTA's warps leave at once
+    const size_t qpc = blockDim.x >> 1;
+    __shared__ g1a gen_sh;
+    if (threadIdx.x == 0) { fp_set(gen_sh.x, K_G1_X); fp_set(gen_sh.y, K_G1_Y); }
+    __syncthreads();
+    for (size_t it = 0; ; it++) {
+        const size_t warp_first = (it * qpc + ((threadIdx.x & ~31u) >> 1)) * gridDim.x + blockIdx.x;
+        if (warp_first >= n) break;
+        const size_t i = (it * qpc + (threadIdx.x >> 1)) * gridDim.x + blockIdx.x;
+        const bool valid = i < n;
+        const size_t g = list[valid ? i : n - 1];
+        const fp* s4 = reinterpret_cast<const fp*>(&Sg[g]);
+        fp2h qx[1], qy[1]; qx[0].c = s4[role]; qy[0].c = s4[2 + role];
+        const bool zx = fp2_is_zero(qx[0]), zy = fp2_is_zero(qy[0]);     // no short-circuit: fp2_is_zero(fp2h) shuffles across the warp
+        const g1a* ps[1] = {&gen_sh};
+        fp12_t<fp2h> m, f;
+        miller_loop_multi<fp2h, 1>(m, ps, qx, qy);
+        const fp* src = reinterpret_cast<const fp*>(fm + 6 * g) + role;
+        fp2h* fc = reinterpret_cast<fp2h*>(&f);
+        for (int t = 0; t < 6; t++) fc[t].c = src[2 * t];
+        fp12_mul(m, m, f);
+        final_exp(m, m);
+        const bool one = fp12_is_one(m);
+        if (valid && role == 0) group_ok[g] = (one && !(zx & zy)) ? 1 : 0;
+    }
+}
+// which form a call that can use blocks takes.  Calls are asynchronous (the host does not know how the previous one ended), so the
+// choice is made on the device: *form = 1 when the last such call had at least one failed group in 64 (k_rlc_form_update).  Then most
+// blocks would fail and the per-group check of their groups -- a Miller loop and a final exponentiation per group at partial occupancy --
+// costs more than the blocks save, so the groups are checked one by one.  gates[0] = ng runs the group form's kernels (their count),
+// gates[1] = ng the block form's; the other is 0.  force_blocks: hbls_set_param("rlc_block", 1).
+__global__ void k_rlc_form(size_t ng, int force_blocks, const int* form, unsigned* gates) {
+    if (HB_TID != 0) return;
+    const bool groups = !force_blocks && *form != 0;
+    gates[0] = groups ? (unsigned)ng : 0u; gates[1] = groups ? 0u : (unsigned)ng;
+}
+__global__ void k_rlc_form_update(size_t ng, const unsigned* counts, int* form) {
+    if (HB_TID != 0) return;
+    *form = 64 * (size_t)counts[1] >= ng ? 1 : 0;
 }
 // ---- the EXACT check through the same two kernels: a "group" of ONE round = the pairs (-apk_j, H(m_j)) and (B, sigma_j), i.e.
 // k_rlc_lines_split<1> / k_rlc_accum_split<1> with pk_scaled_neg = -apk (affine) and Sg = the decoded signatures.  These two small
