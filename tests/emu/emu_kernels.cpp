@@ -44,9 +44,12 @@ template <class F> static void run_pair(F f) {                 // one CTA of two
 
 // The aggregate-verify pipeline of hbls.cu (agg_verify_device_locked + launch_verify_tail) with groups of G rounds.
 // mode 1: batched groups + exact fallback, mode 0: exact only.  Returns 0, or -3 if a committee key does not decode.
+// chunk: groups per pass of the line buffer (hbls.cu rlc_chunk_groups(), one wave of the line kernel on the device).  0: the group
+// form in two halves and the exact forms in one pass; > 0: every loop of launch_verify_tail / launch_exact_two_phase over chunks of
+// that many groups, the exact pass over the failed groups' list sized for the worst case (every round) as on the device.
 template <int G> static int aggregate_verify_batch(int mode, uint32_t n, const uint8_t* pks48, size_t B, const uint8_t* bitmaps, size_t blen,
                                           const uint8_t* sigs96, const uint8_t* msgs, uint32_t msg_len, uint64_t s0, uint64_t s1,
-                                          uint8_t* results, int* any_fail_out, uint8_t* group_ok_out, int* groups_failed_out) {
+                                          uint8_t* results, int* any_fail_out, uint8_t* group_ok_out, int* groups_failed_out, size_t chunk) {
     std::vector<g1a> table(n), pkneg(B), pk_scaled(B); std::vector<uint8_t> okk(n), ok_sig(B), ok_hm(B), bad(B), group_ok(B / G + 1);
     std::vector<g1> apk(B); std::vector<g2a> sig(B), hm(B), Sg(B / G + 1); std::vector<g2> S(B);
     run_seq(1, n, [&] { k_g1_decode(n, pks48, table.data(), okk.data(), 1, 0); });
@@ -56,7 +59,7 @@ template <int G> static int aggregate_verify_batch(int mode, uint32_t n, const u
     run_seq(2, 3, [&] { k_mask_aggregate_serial(B, n, table.data(), &total, bitmaps, blen, apk.data()); });     // grid-stride: 6 "threads"
     run_seq(2, 2, [&] { k_g2_decode(B, sigs96, sig.data(), ok_sig.data(), 1); });
     run_seq(3, 1, [&] { k_hash_to_g2(B, msgs, msg_len, hm.data(), ok_hm.data()); });
-    int any_fail = 0; bool two_phase_mismatch = false; std::vector<uint8_t> list_check;
+    int any_fail = 0; bool two_phase_mismatch = false, unwritten = false; std::vector<uint8_t> list_check;
     auto exact = [&](size_t off, size_t cnt, const int* run_if) {
         run_seq(1, (unsigned)cnt, [&] { k_g1_normalize(cnt, apk.data() + off, pkneg.data() + off, 1, run_if); });
         run_pair([&] { k_pairing_verify_split(cnt, sig.data() + off, pkneg.data() + off, hm.data() + off, ok_sig.data() + off, ok_hm.data() + off,
@@ -64,12 +67,17 @@ template <int G> static int aggregate_verify_batch(int mode, uint32_t n, const u
         run_seq(1, 2, [&] { k_pairing_fixup(cnt, sig.data() + off, pkneg.data() + off, hm.data() + off, ok_sig.data() + off, ok_hm.data() + off,
                                             (const uint8_t*)nullptr, results + off, run_if); });
         if (run_if == nullptr && cnt) {      // the same verdicts through the line / accumulator kernels with "groups" of one round (hbls.cu launch_exact_two_phase)
+            const size_t W = chunk ? chunk : cnt;
             std::vector<uint8_t> bad1(cnt), verdict(cnt, 0xee), res2(cnt, 0xee);
-            std::vector<fp> lines((size_t)HB_ML_STEPS * 3 * 2 * cnt * 2);
+            std::vector<fp> lines((size_t)HB_ML_STEPS * 3 * 2 * (W < cnt ? W : cnt) * 2);          // one chunk's lines, reused
             run_seq(1, (unsigned)cnt, [&] { k_exact_prepare(cnt, (const uint32_t*)nullptr, sig.data() + off, pkneg.data() + off, hm.data() + off, ok_sig.data() + off, ok_hm.data() + off,
                                                             (const uint8_t*)nullptr, (g1a*)nullptr, (g2a*)nullptr, (g2a*)nullptr, bad1.data(), res2.data()); });
-            run_pair([&] { k_rlc_lines_split<1>(cnt, 0, cnt, pkneg.data() + off, hm.data() + off, sig.data() + off, lines.data()); });
-            run_pair([&] { k_rlc_accum_split<1>(cnt, 0, cnt, lines.data(), bad1.data(), verdict.data()); });
+            for (size_t g0 = 0; g0 < cnt; g0 += W) {
+                const size_t nc = cnt - g0 < W ? cnt - g0 : W;
+                run_pair([&] { k_rlc_lines_split<1>(cnt, g0, nc, pkneg.data() + off, hm.data() + off, sig.data() + off, lines.data()); });
+                run_pair([&] { k_rlc_accum_split<1>(cnt, g0, nc, lines.data(), bad1.data(), verdict.data()); });
+            }
+            for (size_t t = 0; t < cnt; t++) unwritten |= verdict[t] == 0xee;
             run_seq(1, (unsigned)cnt, [&] { k_exact_publish(cnt, (const uint32_t*)nullptr, verdict.data(), res2.data()); });
             run_seq(1, 2, [&] { k_pairing_fixup(cnt, sig.data() + off, pkneg.data() + off, hm.data() + off, ok_sig.data() + off, ok_hm.data() + off,
                                                 (const uint8_t*)nullptr, res2.data(), (const int*)nullptr); });
@@ -90,12 +98,12 @@ template <int G> static int aggregate_verify_batch(int mode, uint32_t n, const u
         }
         run_seq(1, 2, [&] { k_rlc_group_sum<G>(ng, S.data(), Sg.data()); });
         run_pair([&] { k_rlc_pairing_split<G>(ng, pk_scaled.data(), hm.data(), Sg.data(), bad.data(), group_ok.data()); });
-        {   // the two-kernel form (lines to memory, then the accumulator) must give the same verdicts -- in two chunks, like a large batch
+        {   // the two-kernel form (lines to memory, then the accumulator) must give the same verdicts -- in chunks, like a large batch
             std::vector<uint8_t> gok2(ng + 1, 0xee);
-            const size_t half = ng / 2 ? ng / 2 : ng;
-            for (size_t g0 = 0; g0 < ng; g0 += half) {
-                const size_t ngc = ng - g0 < half ? ng - g0 : half;
-                std::vector<fp> lines((size_t)HB_ML_STEPS * 3 * (G + 1) * ngc * 2);
+            const size_t W = chunk ? chunk : (ng / 2 ? ng / 2 : ng);
+            std::vector<fp> lines((size_t)HB_ML_STEPS * 3 * (G + 1) * (W < ng ? W : ng) * 2);    // one chunk's lines, reused
+            for (size_t g0 = 0; g0 < ng; g0 += W) {
+                const size_t ngc = ng - g0 < W ? ng - g0 : W;
                 run_pair([&] { k_rlc_lines_split<G>(ng, g0, ngc, pk_scaled.data(), hm.data(), Sg.data(), lines.data()); });
                 run_pair([&] { k_rlc_accum_split<G>(ng, g0, ngc, lines.data(), bad.data(), gok2.data()); });
             }
@@ -106,15 +114,22 @@ template <int G> static int aggregate_verify_batch(int mode, uint32_t n, const u
         run_seq(1, 3, [&] { k_g1_normalize_list(&counts[0], list.data(), apk.data(), pkneg.data(), 1); });
         run_pair([&] { k_pairing_verify_split_list(&counts[0], list.data(), sig.data(), pkneg.data(), hm.data(), ok_sig.data(), ok_hm.data(), (const uint8_t*)nullptr, results); });
         std::vector<uint8_t> res_before(results, results + B);
-        {   // the list through the line / accumulator kernels (gathered "groups" of one round, device-side count): same verdicts
+        {   // the list through the line / accumulator kernels (gathered "groups" of one round, device-side count): same verdicts.  The
+            // host loops over the worst case, nr listed rounds; chunks at or past the count must return at once and write nothing
             std::vector<uint8_t> res2(B); std::vector<uint32_t> list2(B); unsigned counts2[2] = {0, 0};
             run_seq(2, (unsigned)((nr + 1) / 2), [&] { k_rlc_finish(nr, ng, group_ok.data(), res2.data(), list2.data(), counts2); });
+            const size_t W = chunk ? chunk : nr;
             std::vector<g1a> pk_c(B); std::vector<g2a> hm_c(B), sig_c(B); std::vector<uint8_t> bad1(B, 0), verdict(B, 0xee);
-            std::vector<fp> lines((size_t)HB_ML_STEPS * 3 * 2 * (nr ? nr : 1) * 2);
+            std::vector<fp> lines((size_t)HB_ML_STEPS * 3 * 2 * (W < nr ? W : nr) * 2);
             run_seq(1, (unsigned)nr, [&] { k_exact_prepare(nr, list2.data(), sig.data(), pkneg.data(), hm.data(), ok_sig.data(), ok_hm.data(), (const uint8_t*)nullptr,
                                                            pk_c.data(), hm_c.data(), sig_c.data(), bad1.data(), res2.data(), &counts2[0]); });
-            run_pair([&] { k_rlc_lines_split<1>(nr, 0, nr, pk_c.data(), hm_c.data(), sig_c.data(), lines.data(), &counts2[0]); });
-            run_pair([&] { k_rlc_accum_split<1>(nr, 0, nr, lines.data(), bad1.data(), verdict.data(), &counts2[0]); });
+            for (size_t g0 = 0; g0 < nr; g0 += W) {
+                const size_t nc = nr - g0 < W ? nr - g0 : W;
+                run_pair([&] { k_rlc_lines_split<1>(nr, g0, nc, pk_c.data(), hm_c.data(), sig_c.data(), lines.data(), &counts2[0]); });
+                run_pair([&] { k_rlc_accum_split<1>(nr, g0, nc, lines.data(), bad1.data(), verdict.data(), &counts2[0]); });
+            }
+            for (size_t t = 0; t < counts2[0]; t++) unwritten |= verdict[t] == 0xee;
+            for (size_t t = counts2[0]; t < B; t++) if (verdict[t] != 0xee) return -10;       // written past the device-side count
             run_seq(1, (unsigned)nr, [&] { k_exact_publish(nr, list2.data(), verdict.data(), res2.data(), &counts2[0]); });
             run_seq(1, 2, [&] { k_pairing_fixup_list(&counts2[0], list2.data(), sig.data(), pkneg.data(), hm.data(), ok_sig.data(), ok_hm.data(), (const uint8_t*)nullptr, res2.data()); });
             list_check = std::move(res2);
@@ -129,14 +144,15 @@ template <int G> static int aggregate_verify_batch(int mode, uint32_t n, const u
         exact(0, B, nullptr);
     }
     if (any_fail_out) *any_fail_out = any_fail;
+    if (unwritten) return -11;              // a round of the exact two-kernel forms got no verdict (a chunk skipped or cut short)
     if (two_phase_mismatch) return -7;
     return 0;
 }
 extern "C" int emu_aggregate_verify_batch(int mode, uint32_t n, const uint8_t* pks48, size_t B, const uint8_t* bitmaps, size_t blen,
                                           const uint8_t* sigs96, const uint8_t* msgs, uint32_t msg_len, uint64_t s0, uint64_t s1,
-                                          uint8_t* results, int* any_fail_out, uint8_t* group_ok_out, int G, int* groups_failed_out) {
-    return G == 8 ? aggregate_verify_batch<8>(mode, n, pks48, B, bitmaps, blen, sigs96, msgs, msg_len, s0, s1, results, any_fail_out, group_ok_out, groups_failed_out)
-                  : aggregate_verify_batch<4>(mode, n, pks48, B, bitmaps, blen, sigs96, msgs, msg_len, s0, s1, results, any_fail_out, group_ok_out, groups_failed_out);
+                                          uint8_t* results, int* any_fail_out, uint8_t* group_ok_out, int G, int* groups_failed_out, size_t chunk) {
+    return G == 8 ? aggregate_verify_batch<8>(mode, n, pks48, B, bitmaps, blen, sigs96, msgs, msg_len, s0, s1, results, any_fail_out, group_ok_out, groups_failed_out, chunk)
+                  : aggregate_verify_batch<4>(mode, n, pks48, B, bitmaps, blen, sigs96, msgs, msg_len, s0, s1, results, any_fail_out, group_ok_out, groups_failed_out, chunk);
 }
 
 // Executed Fp multiplications / squarings of the thread-per-item stages (mask aggregation from the complement side, signature

@@ -24,7 +24,8 @@ def emuk(request):
     L = ctypes.CDLL(out)
     L.emu_aggregate_verify_batch.argtypes = [ctypes.c_int, ctypes.c_uint32, ctypes.c_char_p, ctypes.c_size_t, ctypes.c_char_p, ctypes.c_size_t,
                                              ctypes.c_char_p, ctypes.c_char_p, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_uint64,
-                                             ctypes.c_char_p, ctypes.POINTER(ctypes.c_int), ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]
+                                             ctypes.c_char_p, ctypes.POINTER(ctypes.c_int), ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int),
+                                             ctypes.c_size_t]
     return L
 
 @pytest.fixture(scope="module")
@@ -49,12 +50,16 @@ def make_batch(oracle, n, B, seed):
         bitmaps.append(bytes(bm)); msgs.append(m); sigs.append(oracle.sign_hash(wl.sk_bytes(agg_sk), m))
     return pks, blen, bitmaps, sigs, msgs
 
-def run(emuk, mode, pks, blen, bitmaps, sigs, msgs, seed=(0x1234, 0x9876), G=4):
+def run_info(emuk, mode, pks, blen, bitmaps, sigs, msgs, seed=(0x1234, 0x9876), G=4, chunk=0):
+    """-> per-round results, any round listed, per-group verdicts, groups failed.  chunk > 0: groups per pass of the line buffer."""
     B = len(sigs); res = ctypes.create_string_buffer(B); gok = ctypes.create_string_buffer(B // 4 + 1); af = ctypes.c_int(-1); gf = ctypes.c_int(-1)
     rc = emuk.emu_aggregate_verify_batch(mode, len(pks), b"".join(pks), B, b"".join(bitmaps), blen, b"".join(sigs), b"".join(msgs), 48,
-                                         seed[0], seed[1], res, ctypes.byref(af), gok, G, ctypes.byref(gf))
-    assert rc == 0
-    return res.raw[:B], af.value, gok.raw[:B // G]
+                                         seed[0], seed[1], res, ctypes.byref(af), gok, G, ctypes.byref(gf), chunk)
+    assert rc == 0, rc
+    return res.raw[:B], af.value, gok.raw[:B // G], gf.value
+
+def run(emuk, mode, pks, blen, bitmaps, sigs, msgs, seed=(0x1234, 0x9876), G=4):
+    return run_info(emuk, mode, pks, blen, bitmaps, sigs, msgs, seed, G)[:3]
 
 def expected(oracle, pks, bitmaps, sigs, msgs):
     h = oracle.committee(pks)
@@ -95,6 +100,72 @@ def test_pipeline_groups_of_eight(emuk, oracle):
     want = expected(oracle, pks, bitmaps, sigs, msgs)
     res, any_fail, gok = run(emuk, 1, pks, blen, bitmaps, sigs, msgs, G=8)
     assert gok == b"\x00\x01" and any_fail == 1 and res == want and want[4] == 0 and sum(want) == 16
+
+# ---- batches beyond one chunk of the line buffer.  On the device a chunk is rlc_chunk_groups() = SM count x 256 groups; here it is a
+# few groups, so that the group form, the exact pass over the failed groups' list and the exact form each run over several chunks.
+# Groups are strided: round (k, g) = k * ng + g.
+def rnd(ng, k, g):
+    return k * ng + g
+
+def flip(msg):
+    return bytes([msg[0] ^ 1]) + msg[1:]
+
+def check_chunked(emuk, oracle, pks, blen, bitmaps, sigs, msgs, G, chunk, bad):
+    """The batch in chunks of `chunk` groups (the exact forms: `chunk` rounds) gives the oracle's verdicts, which are 0 exactly at the
+    injected rounds, and the group verdicts, groups_failed and results of the same pipeline in one pass; exact mode in chunks agrees."""
+    B = len(sigs); ng = B // G
+    want = expected(oracle, pks, bitmaps, sigs, msgs)
+    assert {j for j in range(B) if want[j] != 1} == set(bad)
+    failed = {j % ng for j in bad if j < ng * G}
+    one = run_info(emuk, 1, pks, blen, bitmaps, sigs, msgs, G=G)
+    got = run_info(emuk, 1, pks, blen, bitmaps, sigs, msgs, G=G, chunk=chunk)
+    assert got == one
+    assert got[0] == want and got[1] == (1 if failed else 0) and got[3] == len(failed)
+    assert got[2] == bytes(0 if g in failed else 1 for g in range(ng))
+    assert run_info(emuk, 0, pks, blen, bitmaps, sigs, msgs, G=G, chunk=chunk)[0] == want
+
+@pytest.mark.parametrize("G", [4, 8])
+def test_chunked_irregular_rounds_at_chunk_edges(emuk, oracle, G):
+    """7 groups in chunks of 3 (3 + 3 + 1: the last chunk holds one group) and a tail of 2.  A wrong message, an undecodable signature,
+    an identity signature, an empty bitmap and another round's signature sit in the first and last group of every chunk, and a wrong
+    message in the middle of the first chunk.  Group 4 is the only clean group.  The failed groups' list (6 G rounds) runs in chunks of
+    3 rounds, and the loop over the worst case (7 G rounds) runs past it."""
+    ng = 7
+    pks, blen, bitmaps, sigs, msgs = make_batch(oracle, 10, ng * G + 2, seed=40 + G)
+    bad = {rnd(ng, 0, 0), rnd(ng, G - 1, 2), rnd(ng, 0, 3), rnd(ng, G - 1, 5), rnd(ng, 1, 6), rnd(ng, 2, 1), ng * G, ng * G + 1}
+    msgs[rnd(ng, 0, 0)] = flip(msgs[rnd(ng, 0, 0)])                 # first group of chunk 0
+    sigs[rnd(ng, G - 1, 2)] = b"\xff" * 96                          # last group of chunk 0: does not decode
+    sigs[rnd(ng, 0, 3)] = bytes(96)                                 # first group of chunk 1: identity signature
+    bitmaps[rnd(ng, G - 1, 5)] = bytes(blen)                        # last group of chunk 1: empty bitmap (identity aggregate key)
+    sigs[rnd(ng, 1, 6)] = sigs[rnd(ng, 0, 1)]                       # the one-group chunk: a valid point of another round
+    msgs[rnd(ng, 2, 1)] = flip(msgs[rnd(ng, 2, 1)])                 # middle of chunk 0
+    sigs[ng * G] = bytes(96); msgs[ng * G + 1] = flip(msgs[ng * G + 1])     # tail
+    check_chunked(emuk, oracle, pks, blen, bitmaps, sigs, msgs, G, 3, bad)
+
+@pytest.mark.parametrize("G", [4, 8])
+def test_chunked_list_spans_three_chunks_and_a_partial_one(emuk, oracle, G):
+    """16 listed rounds (4 failed groups of 4, or 2 of 8) in chunks of 5: 5 + 5 + 5 + 1; the group form in chunks of 5 groups (5 + 2)."""
+    ng = 7
+    pks, blen, bitmaps, sigs, msgs = make_batch(oracle, 10, ng * G + 1, seed=50 + G)
+    groups = [0, 2, 4, 6] if G == 4 else [1, 5]
+    bad = {rnd(ng, (3 * i + 1) % G, g) for i, g in enumerate(groups)}
+    for j in bad: msgs[j] = flip(msgs[j])
+    check_chunked(emuk, oracle, pks, blen, bitmaps, sigs, msgs, G, 5, bad)
+
+@pytest.mark.parametrize("G", [4, 8])
+def test_chunked_list_shorter_than_a_chunk(emuk, oracle, G):
+    """One failed group: G listed rounds, less than a chunk of G + 2, while the loop over the worst case (7 G rounds) runs 5 or 6 chunks."""
+    ng = 7
+    pks, blen, bitmaps, sigs, msgs = make_batch(oracle, 10, ng * G + 1, seed=60 + G)
+    j = rnd(ng, G - 1, ng - 1)
+    msgs[j] = flip(msgs[j])
+    check_chunked(emuk, oracle, pks, blen, bitmaps, sigs, msgs, G, G + 2, {j})
+
+@pytest.mark.parametrize("G", [4, 8])
+def test_chunked_empty_list(emuk, oracle, G):
+    """All valid: the list is empty and every chunk of the exact pass must return at once (chunks of 2)."""
+    pks, blen, bitmaps, sigs, msgs = make_batch(oracle, 10, 7 * G + 3, seed=70 + G)
+    check_chunked(emuk, oracle, pks, blen, bitmaps, sigs, msgs, G, 2, set())
 
 def test_stage_counts_pinned(emuk, oracle, request):
     """bench.py's roofline counts EXECUTED Fp multiplications / squarings per round for every stage; the figures are those of the
