@@ -117,6 +117,7 @@ def lib():
         sig("hbls_ballot_box_destroy", None, vp)
         sig("hbls_ballot_box_add_vote", c.c_int, vp, u8p, sz, u8p)
         sig("hbls_ballot_box_aggregate", c.c_int, vp, vp, vp, sz)
+        sig("hbls_ballot_box_submit_votes", c.c_int, vp, sz, vp, sz, vp, u8p, sz, vp)
         sig("hbls_selftest_split", c.c_int, c.c_uint32)
         sig("hbls_set_batch_mode", None, c.c_int)
         sig("hbls_get_batch_mode", c.c_int)
@@ -550,6 +551,10 @@ class DeviceMask:
         if rc < 0: raise HblsError(f"hbls_mask_verify rc={rc}")
         return rc == 1
 
+# hbls_ballot_box_submit_votes statuses, in the order onPrepare / onCommit meet the errors (include/hbls.h)
+BALLOT_ACCEPTED, BALLOT_COLLECTED, BALLOT_BAD_SIG_ENCODING, BALLOT_BAD_SIG = 16, 17, 18, 19
+BALLOT_MAX_BITMAP_BYTES = 2048                                  # committees of up to 16 384 slots (include/hbls.h)
+
 class BallotBox:
     """Running vote aggregate (hbls_ballot_box_*): quorum.go:164-196 AggregateVotes with each vote decoded once on arrival."""
     def __init__(self, committee: Committee):
@@ -566,6 +571,21 @@ class BallotBox:
         if rc == ERR_DECODE: raise ValueError("err blsSignatureDeserialize")
         if rc < 0: raise HblsError(f"hbls_ballot_box_add_vote rc={rc}")
         return rc == 0
+    def SubmitVotes(self, bitmaps, sigs96, msg: bytes) -> bytes:
+        """A leader's queue of votes on msg in one device call (hbls_ballot_box_submit_votes): bitmaps = the votes' signer bitmaps
+        (a list, or their concatenation), sigs96 likewise.  One BALLOT_* status per vote, decided in arrival order."""
+        bm = b"".join(bytes(b) for b in bitmaps) if isinstance(bitmaps, (list, tuple)) else bytes(bitmaps)
+        sg = b"".join(bytes(s) for s in sigs96) if isinstance(sigs96, (list, tuple)) else bytes(sigs96)
+        blen = self.c.blen(); k = len(sg) // 96
+        if len(sg) != 96 * k or len(bm) != k * blen:
+            raise ValueError(f"{k} votes need {k * blen} bitmap bytes (got {len(bm)}) and {96 * k} signature bytes (got {len(sg)})")
+        if len(msg) > 64: raise ValueError(f"message of {len(msg)} bytes: at most 64 (only the first 48 enter H(m))")
+        if blen > BALLOT_MAX_BITMAP_BYTES: raise ValueError(f"committee of {self.c.n} slots: a vote queue takes at most {8 * BALLOT_MAX_BITMAP_BYTES}")
+        st = ctypes.create_string_buffer(k if k else 1)
+        rc = _lib.hbls_ballot_box_submit_votes(self.h, k, _buf(bm), blen, _buf(sg), _buf(msg), len(msg), st)
+        if rc == ERR_ARG: raise ValueError("hbls_ballot_box_submit_votes: bad argument")
+        if rc != 0: raise HblsError(f"hbls_ballot_box_submit_votes rc={rc}")
+        return st.raw[:k]
     def Aggregate(self):
         sig = ctypes.create_string_buffer(96); bm = ctypes.create_string_buffer(self.c.blen() if self.c.blen() else 1)
         rc = _lib.hbls_ballot_box_aggregate(self.h, sig, bm, self.c.blen())

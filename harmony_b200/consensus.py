@@ -383,3 +383,105 @@ class VoteCollector:
             if any(k in seen for k in keys): continue
             seen.update(keys); sigs.append(sig)
         return (self.be.aggregate_sigs(sigs) if sigs else bytes(96)), bytes(self.bitmap)
+
+class BoxBackend(DeviceBackend):
+    """DeviceBackend plus the device ballot box that BallotBoxCollector collects into."""
+    def ballot_box(self, com): return bls.BallotBox(com)
+
+_UNDECODABLE = b"\xff" * 96             # x >= p: stands in for a payload of the wrong length, which Sign.Deserialize rejects too
+
+class BallotBoxCollector:
+    """VoteCollector's interface and results, collected into a device ballot box (hbls_ballot_box_submit_votes).  The leader maps
+    sender keys to committee slots on the host; a queue whose votes each name distinct committee members goes to the device in ONE
+    call -- signer keys summed from the committee table (no key decoded), H(m) hashed once, the already-received / Deserialize /
+    VerifyHash rules applied in arrival order on the device, accepted signatures folded into the box's running sum without being
+    decoded again.  A vote with a repeated key, a non-member key or a key held by a ballot without a bit (below) cuts the queue there
+    and goes through VoteCollector's path (key sum, status triple); honest queues never hold one.
+    The reference records a ballot of a non-member key (decider.AddNewVote) before bitmap.SetKeysAtomic fails (leader.go:185-196), so
+    its signature counts in AggregateVotes without a bit: such a ballot enters the box with an empty bitmap, and its keys are kept
+    here so that a later vote by one of them is "already received"."""
+    def __init__(self, members: List[bytes], message: bytes, backend=None):
+        self.members = [bytes(m) for m in members]
+        self.index = {m: i for i, m in enumerate(self.members)}
+        self.message = bytes(message)
+        self.be = backend or BoxBackend()
+        self.blen = (len(self.members) + 7) >> 3
+        self.quorum = 2 * len(self.members) // 3 + 1            # uniform vote: TwoThirdsSignersCount (quorum.go:409-411)
+        self.box = self.be.ballot_box(self.be.committee(self.members))
+        self.BallotBox = {}                                       # votepower.Round.BallotBox: key -> (SignerPubKeys, Signature)
+        self.unbitted = set()                                     # keys of ballots recorded without a bit
+    def SignersCount(self) -> int: return len(self.BallotBox)
+    def IsQuorumAchieved(self) -> bool: return self.SignersCount() >= self.quorum
+    def _slots(self, v):
+        """the vote's committee slots when the device can judge it alone, else None"""
+        keys = [bytes(k) for k in v.SenderPubkeys]
+        if not keys or len(set(keys)) != len(keys): return None
+        if any(k not in self.index or k in self.unbitted for k in keys): return None
+        return [self.index[k] for k in keys]
+    def onVotes(self, votes: List[Vote]):
+        """(errors, quorum_at) exactly as VoteCollector.onVotes."""
+        n = len(votes)
+        out, quorum_at = [None] * n, None
+        i = 0
+        while i < n:
+            j, slots = i, []
+            while j < n:
+                s = self._slots(votes[j])
+                if s is None: break
+                slots.append(s); j += 1
+            errs = self._device(votes[i:j], slots) if j > i else []
+            if j < n: errs.append(self._irregular(votes[j])); j += 1
+            for t, e in enumerate(errs):
+                out[i + t] = e
+            i = j
+        # quorum transition, vote by vote (a vote changes the count only when it is counted)
+        count = self.SignersCount() - sum(len(votes[t].SenderPubkeys) for t in range(n) if out[t] in (None, errKeyNotFound))
+        for t in range(n):
+            was = count >= self.quorum
+            if out[t] in (None, errKeyNotFound): count += len(votes[t].SenderPubkeys)
+            if out[t] is None and not was and count >= self.quorum and quorum_at is None: quorum_at = t
+        return out, quorum_at
+    def _device(self, votes, slots):
+        bms = []
+        for s in slots:
+            bm = bytearray(self.blen)
+            for x in s: bm[x >> 3] |= 1 << (x & 7)
+            bms.append(bytes(bm))
+        sigs = [bytes(v.Payload) if len(v.Payload) == 96 else _UNDECODABLE for v in votes]
+        st = self.box.SubmitVotes(bms, sigs, _m48(self.message))             # what H(m) reads, as VoteCollector's backend passes it
+        errs = []
+        for v, s in zip(votes, st):
+            if s == bls.BALLOT_ACCEPTED:
+                keys = [bytes(k) for k in v.SenderPubkeys]
+                for k in keys: self.BallotBox[k] = (keys, bytes(v.Payload))
+                errs.append(None)
+            else:
+                errs.append(errAlreadyReceived if s == bls.BALLOT_COLLECTED else errSigDeserialize if s == bls.BALLOT_BAD_SIG_ENCODING else errVoteSig)
+        return errs
+    def _irregular(self, v):
+        """VoteCollector's path for one vote (key sum, status triple, the reference's checks in order)"""
+        keys = [bytes(k) for k in v.SenderPubkeys]
+        pk, pre = bytes(48), None
+        if len(keys) == 1 and len(keys[0]) == 48: pk = keys[0]
+        elif len(keys) > 1:
+            try: pk = self.be.aggregate_keys(keys)
+            except ValueError: pre = errKeyDeserialize
+        else: pre = errKeyDeserialize
+        st = self.be.verify_status([pk], [bytes(v.Payload) if len(v.Payload) == 96 else bytes(96)], [self.message])[0]
+        if pre is not None or st == bls.VB_BAD_KEY_ENCODING: return errKeyDeserialize
+        if any(k in self.BallotBox for k in keys): return errAlreadyReceived
+        if len(v.Payload) != 96 or st == bls.VB_BAD_SIG_ENCODING: return errSigDeserialize
+        if st != bls.VB_OK: return errVoteSig
+        if len(set(keys)) != len(keys): return errDuplicateKey
+        for k in keys: self.BallotBox[k] = (keys, bytes(v.Payload))
+        member = all(k in self.index for k in keys)
+        bm = bytearray(self.blen)
+        if member:
+            for k in keys: i = self.index[k]; bm[i >> 3] |= 1 << (i & 7)
+        else: self.unbitted.update(keys)
+        self.box.AddVote(bytes(bm), bytes(v.Payload))
+        return None if member else errKeyNotFound
+    def AggregateVotes(self):
+        """(aggregate signature, bitmap) of the collected ballots: the device box's running sum and bitmap (quorum.go:164-196)."""
+        sig, bm = self.box.Aggregate()
+        return (sig if self.BallotBox else bytes(96)), bm

@@ -1401,6 +1401,45 @@ int hbls_ballot_box_add_vote(hbls_ballot_box* b, const uint8_t* signer_bitmap, s
     std::lock_guard<std::mutex> lk(g.mu);
     return ballot_box_add_vote_locked(b, signer_bitmap, blen, sig96);
 }
+static_assert(HB_BALLOT_ACCEPTED == HBLS_BALLOT_ACCEPTED && HB_BALLOT_COLLECTED == HBLS_BALLOT_COLLECTED &&
+              HB_BALLOT_BAD_SIG_ENCODING == HBLS_BALLOT_BAD_SIG_ENCODING && HB_BALLOT_BAD_SIG == HBLS_BALLOT_BAD_SIG, "ballot status codes");
+// a leader's vote queue: same-message aggregate verification over the committee table (mask aggregation, signature decode, H(m)
+// once), then the ballot rules in arrival order and the fold of the accepted signatures, all on the device.  One H2D copy of the box's
+// bitmap and the queue, one D2H copy of the statuses and the new bitmap, one synchronise.
+static int ballot_box_submit_votes_locked(hbls_ballot_box* b, size_t k, const uint8_t* signer_bitmaps, size_t blen, const uint8_t* sigs96,
+                                          const void* msg, size_t msg_len, uint8_t* status) {
+    auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };            // the arena's alignment: offsets of the staged copy
+    const size_t o_sig = up(k * blen), o_col = o_sig + up(k * 96), o_msg = o_col + up(blen), in_bytes = o_msg + msg_len + 1;
+    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(k) + in_bytes + up(k + blen) + up(k) + 4096, &sc)) return e;
+    ensure_stage_events(sc);
+    Arena ar{sc->base, 0, sc->cap};
+    uint8_t* din = ar.take<uint8_t>(in_bytes); uint8_t* dres = ar.take<uint8_t>(k); uint8_t* dacc = ar.take<uint8_t>(k);
+    uint8_t* dout = ar.take<uint8_t>(k + blen);                             // statuses, then the new collected bitmap
+    std::vector<uint8_t> h(in_bytes, 0);
+    memcpy(h.data(), signer_bitmaps, k * blen); memcpy(h.data() + o_sig, sigs96, k * 96);
+    memcpy(h.data() + o_col, b->collected.data(), blen); if (msg_len) memcpy(h.data() + o_msg, msg, msg_len);
+    CK(cudaMemcpyAsync(din, h.data(), in_bytes, cudaMemcpyHostToDevice, g.stream));
+    VerifyBufs v;
+    agg_verify_device_locked(b->c, k, din, blen, din + o_sig, din + o_msg, msg_len, dres, g.stream, sc, ar, true, &v, (const uint8_t*)msg);
+    LAUNCH(k_ballot_admit, 1, HB_BALLOT_THREADS, g.stream, k, b->c->n, blen, (const uint8_t*)din, (const uint8_t*)dres, (const uint8_t*)v.ok_sig,
+           (const uint8_t*)(din + o_col), dout + k, dout, dacc);
+    LAUNCH(k_ballot_fold, 1, HB_SUM_THREADS, g.stream, k, (const g2a*)v.sig, (const uint8_t*)dacc, b->d_sum);
+    std::vector<uint8_t> back(k + blen);
+    CK(cudaMemcpyAsync(back.data(), dout, k + blen, cudaMemcpyDeviceToHost, g.stream));
+    CK(cudaStreamSynchronize(g.stream));
+    memcpy(status, back.data(), k);
+    memcpy(b->collected.data(), back.data() + k, blen);
+    return 0;
+}
+int hbls_ballot_box_submit_votes(hbls_ballot_box* b, size_t k, const uint8_t* signer_bitmaps, size_t blen, const uint8_t* sigs96,
+                                 const void* msg, size_t msg_len, uint8_t* status) {
+    if (int e = ensure_init()) return e;
+    if (!b || !status || blen != b->collected.size() || msg_len > 64 || blen > HB_BALLOT_MAX_BYTES) return HBLS_ERR_ARG;
+    if (k == 0) return 0;
+    if (!signer_bitmaps || !sigs96 || (msg_len && !msg)) return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return ballot_box_submit_votes_locked(b, k, signer_bitmaps, blen, sigs96, msg, msg_len, status);
+}
 static int ballot_box_aggregate_locked(const hbls_ballot_box* b, uint8_t out_sig96[96], uint8_t* bitmap_out, size_t blen) {
     Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};

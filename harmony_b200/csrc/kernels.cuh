@@ -221,6 +221,77 @@ __global__ void __launch_bounds__(HB_SUM_THREADS) k_g2_sum(size_t n, const g2a* 
     if (threadIdx.x == 0) out[0] = acc;
 }
 
+// ---- leader's vote queue into the ballot box (hbls_ballot_box_submit_votes; consensus/leader.go:110-345, quorum.go:164-196,354-377).
+// k_ballot_admit applies the ballot rules in arrival order: vote j's fate depends on the verdicts of the votes before it, so one CTA
+// walks the queue with the box's collected bitmap in shared memory.  Votes are staged into shared memory a chunk at a time (one
+// coalesced load per chunk); per vote, each thread tests its bytes of the bitmap against the box and the CTA meets at ONE barrier.
+// The "some signer is already collected" flag is a stamp (j + 1) in a slot that alternates with j, so it never needs clearing: a
+// thread that writes vote j + 1's slot has passed vote j's barrier, hence every thread has left vote j - 1, the slot's last reader.
+// Statuses follow the order in which onPrepare / onCommit meet the errors: already collected (before the signature is looked at),
+// signature does not decode, VerifyHash false, accepted.  Padding bits of the last byte (slots >= n) are ignored.  Any block size
+// (the host emulation runs one thread).
+#define HB_BALLOT_THREADS 128
+#ifndef HB_BALLOT_MAX_BYTES
+#define HB_BALLOT_MAX_BYTES 2048            // collected bitmap held in shared memory: committees of up to 16 384 slots
+#endif
+#ifndef HB_BALLOT_STAGE
+#define HB_BALLOT_STAGE 8192                // staged vote bitmaps per chunk (bytes; the host emulation shrinks both to test chunking)
+#endif
+static_assert(HB_BALLOT_STAGE >= HB_BALLOT_MAX_BYTES, "a chunk holds at least one vote");
+#define HB_BALLOT_CHUNK 1024                // votes per chunk at most
+enum { HB_BALLOT_ACCEPTED = 16, HB_BALLOT_COLLECTED = 17, HB_BALLOT_BAD_SIG_ENCODING = 18, HB_BALLOT_BAD_SIG = 19 };      // == HBLS_BALLOT_*
+__global__ void __launch_bounds__(HB_BALLOT_THREADS) k_ballot_admit(size_t k, size_t n, size_t blen, const uint8_t* __restrict__ bitmaps,
+                                                                   const uint8_t* __restrict__ verified, const uint8_t* __restrict__ ok_sig,
+                                                                   const uint8_t* __restrict__ collected_in, uint8_t* collected_out,
+                                                                   uint8_t* status, uint8_t* accept) {
+    __shared__ uint8_t box[HB_BALLOT_MAX_BYTES];
+    __shared__ uint8_t stage[HB_BALLOT_STAGE];
+    __shared__ uint8_t verdict[HB_BALLOT_CHUNK];        // bit 0: signature decoded, bit 1: VerifyHash true
+    __shared__ uint32_t hit[2];
+    const uint8_t last = (n & 7) ? (uint8_t)((1u << (n & 7)) - 1u) : (uint8_t)0xff;
+    for (size_t i = threadIdx.x; i < blen; i += blockDim.x) box[i] = collected_in[i] & (i + 1 == blen ? last : (uint8_t)0xff);
+    if (threadIdx.x == 0) { hit[0] = 0; hit[1] = 0; }
+    size_t per = HB_BALLOT_STAGE / (blen ? blen : 1);
+    if (per > HB_BALLOT_CHUNK) per = HB_BALLOT_CHUNK;
+    for (size_t j0 = 0; j0 < k; j0 += per) {
+        const size_t m = k - j0 < per ? k - j0 : per;
+        __syncthreads();                                 // the previous chunk's scan is over
+        for (size_t i = threadIdx.x; i < m * blen; i += blockDim.x) stage[i] = bitmaps[j0 * blen + i];
+        for (size_t i = threadIdx.x; i < m; i += blockDim.x) verdict[i] = (uint8_t)((ok_sig[j0 + i] ? 1 : 0) | (verified[j0 + i] ? 2 : 0));
+        __syncthreads();
+        for (size_t t = 0; t < m; t++) {
+            const size_t j = j0 + t;
+            const uint8_t* bm = stage + t * blen;
+            for (size_t i = threadIdx.x; i < blen; i += blockDim.x)
+                if (bm[i] & box[i]) hit[j & 1] = (uint32_t)(j + 1);
+            __syncthreads();
+            const bool dup = hit[j & 1] == (uint32_t)(j + 1);
+            const uint8_t vd = verdict[t];
+            const bool ok = !dup && vd == 3;
+            if (ok)                                      // each thread ORs the bytes it tests: no barrier needed before the next vote
+                for (size_t i = threadIdx.x; i < blen; i += blockDim.x) box[i] |= bm[i] & (i + 1 == blen ? last : (uint8_t)0xff);
+            if (threadIdx.x == 0) {
+                status[j] = dup ? HB_BALLOT_COLLECTED : !(vd & 1) ? HB_BALLOT_BAD_SIG_ENCODING : !(vd & 2) ? HB_BALLOT_BAD_SIG : HB_BALLOT_ACCEPTED;
+                accept[j] = ok ? 1 : 0;
+            }
+        }
+    }
+    for (size_t i = threadIdx.x; i < blen; i += blockDim.x) collected_out[i] = box[i];
+}
+// the accepted votes' decoded signatures added into the box's running sum (single CTA; block size a power of two, any including 1)
+__global__ void __launch_bounds__(HB_SUM_THREADS) k_ballot_fold(size_t k, const g2a* __restrict__ sig, const uint8_t* __restrict__ accept, g2* sum) {
+    __shared__ g2 sm[HB_SUM_THREADS];
+    g2 acc; pt_set_inf(acc);
+    for (size_t j = threadIdx.x; j < k; j += blockDim.x) if (accept[j]) { g2a q = sig[j]; pt_add_mixed(acc, acc, q); }
+    sm[threadIdx.x] = acc;
+    __syncthreads();
+    for (unsigned off = blockDim.x / 2; off >= 1; off >>= 1) {
+        if (threadIdx.x < off) { g2 o = sm[threadIdx.x + off]; pt_add(acc, acc, o); sm[threadIdx.x] = acc; }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) { g2 s = *sum; pt_add(s, s, acc); *sum = s; }
+}
+
 // ---- message -> G2 (hash part of R6/R7), affine output
 // HB_BATCH_INV: a persistent thread shares ONE inversion among HB_BATCH_K of its items (Montgomery's trick) -- both inversions of
 // hash-to-G2 and the affine conversion of the coefficient-scaling stage: one inversion costs ~400 products, the trick 3 per item.

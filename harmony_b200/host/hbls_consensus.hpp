@@ -351,6 +351,118 @@ private:
         return "";
     }
 };
+
+// VoteCollector's interface and results, collected into a device ballot box (hbls_ballot_box_submit_votes; consensus.py:
+// BallotBoxCollector is the Python twin).  Sender keys are mapped to committee slots on the host; a run of votes that each name
+// distinct committee members goes to the device in ONE call -- keys summed from the committee table (no key decoded), H(m) once, the
+// already-received / Deserialize / VerifyHash rules in arrival order, accepted signatures folded into the box without a second decode.
+// A vote with a repeated key, a non-member key or a key held by a ballot without a bit cuts the queue there and takes VoteCollector's
+// path (key sum, status triple); honest queues never hold one.  The reference records a non-member's ballot (decider.AddNewVote)
+// before bitmap.SetKeysAtomic fails (leader.go:185-196), so its signature counts in AggregateVotes without a bit: it enters the box
+// with an empty bitmap, and its keys are kept here so that a later vote by one of them is "already received".
+class BallotBoxCollector {
+public:
+    using Ballot = VoteCollector::Ballot;
+    std::map<Bytes, Ballot> BallotBox;          // votepower.Round.BallotBox: one entry per signer key
+    Bytes bitmap;                               // the box's bitmap, as the device returned it with the last queue
+    std::string Init(const std::vector<bls::PublicKeyWrapper>& members, const Bytes& message) {
+        index_.clear(); for (size_t i = 0; i < members.size(); i++) index_[Bytes(members[i].Bytes.begin(), members[i].Bytes.end())] = i;
+        message_.clear(); put48(message_, message);                  // what hash-to-G2 reads of the message (VoteCollector: verifyStatus)
+        blen_ = (members.size() + 7) >> 3; bitmap.assign(blen_, 0); BallotBox.clear(); unbitted_.clear();
+        quorum_ = (size_t)quorum::TwoThirdsSignersCount((int64_t)members.size());
+        const std::string e = com_.Load(members);
+        return e.empty() ? box_.Create(com_) : e;
+    }
+    size_t SignersCount() const { return BallotBox.size(); }
+    bool IsQuorumAchieved() const { return SignersCount() >= quorum_; }
+    // errors[i] == "" when vote i was counted; quorumAt = index of the vote that first reached the quorum in this call, or -1
+    std::vector<std::string> onVotes(const std::vector<Vote>& votes, long* quorumAt = nullptr) {
+        const size_t n = votes.size();
+        std::vector<std::string> out(n); if (quorumAt) *quorumAt = -1;
+        size_t i = 0;
+        while (i < n) {
+            size_t j = i; std::vector<std::vector<size_t>> slots;
+            for (std::vector<size_t> s; j < n && slotsOf(votes[j], s); j++) slots.push_back(s);
+            if (j > i) device(votes, i, slots, out);
+            if (j < n) { out[j] = irregular(votes[j]); j++; }
+            i = j;
+        }
+        // the quorum transition, vote by vote: a vote changes the count only when its ballot is recorded
+        auto recorded = [](const std::string& e) { return e.empty() || e == errKeyNotFound; };
+        size_t count = SignersCount();
+        for (size_t t = 0; t < n; t++) if (recorded(out[t])) count -= votes[t].SenderPubkeys.size();
+        for (size_t t = 0; t < n; t++) {
+            const bool was = count >= quorum_;
+            if (recorded(out[t])) count += votes[t].SenderPubkeys.size();
+            if (out[t].empty() && !was && count >= quorum_ && quorumAt && *quorumAt < 0) *quorumAt = (long)t;
+        }
+        return out;
+    }
+    // quorum.go:164-196 from the box: its running sum (all zero when nothing was collected, as VoteCollector) and its bitmap
+    bool AggregateVotes(Bytes& sig) const { Bytes bm; return AggregateVotes(sig, bm); }
+    bool AggregateVotes(Bytes& sig, Bytes& bm) const {
+        if (!box_.Aggregate(sig, bm)) return false;
+        if (BallotBox.empty()) sig.assign(96, 0);
+        return true;
+    }
+private:
+    std::map<Bytes, size_t> index_; std::set<Bytes> unbitted_; Bytes message_; size_t blen_ = 0, quorum_ = 0;
+    bls::Committee com_; bls::BallotBox box_;
+
+    // the vote's committee slots when the device can judge it alone
+    bool slotsOf(const Vote& v, std::vector<size_t>& s) const {
+        s.clear();
+        if (v.SenderPubkeys.empty()) return false;
+        std::set<Bytes> seen;
+        for (auto& k : v.SenderPubkeys) {
+            auto it = index_.find(k);
+            if (it == index_.end() || unbitted_.count(k) || !seen.insert(k).second) return false;
+            s.push_back(it->second);
+        }
+        return true;
+    }
+    void device(const std::vector<Vote>& votes, size_t i0, const std::vector<std::vector<size_t>>& slots, std::vector<std::string>& out) {
+        const size_t k = slots.size();
+        Bytes bms(k * blen_, 0), sigs(96 * k, 0xff);                  // 0xff...: x >= p, stands in for a payload of the wrong length
+        for (size_t t = 0; t < k; t++) {
+            for (size_t x : slots[t]) bms[t * blen_ + (x >> 3)] |= (uint8_t)(1u << (x & 7));
+            const Bytes& p = votes[i0 + t].Payload;
+            if (p.size() == 96) std::memcpy(&sigs[96 * t], p.data(), 96);
+        }
+        std::vector<uint8_t> st;
+        const std::string e = box_.SubmitVotes(bms, sigs, message_, st);
+        if (!e.empty()) throw std::runtime_error(e);
+        for (size_t t = 0; t < k; t++) {
+            const Vote& v = votes[i0 + t];
+            if (st[t] == HBLS_BALLOT_ACCEPTED) {
+                for (auto& key : v.SenderPubkeys) BallotBox[key] = Ballot{v.SenderPubkeys, v.Payload};
+                for (size_t x : slots[t]) bitmap[x >> 3] |= (uint8_t)(1u << (x & 7));
+                out[i0 + t] = "";
+            } else out[i0 + t] = st[t] == HBLS_BALLOT_COLLECTED ? errAlreadyReceived : st[t] == HBLS_BALLOT_BAD_SIG_ENCODING ? errSigDeserialize : errVoteSig;
+        }
+    }
+    // VoteCollector's path for one vote
+    std::string irregular(const Vote& v) {
+        Bytes pk(48, 0); bool keyErr = false;
+        if (v.SenderPubkeys.size() == 1) pk = v.SenderPubkeys[0];
+        else if (v.SenderPubkeys.empty() || !aggregateKeys(v.SenderPubkeys, pk)) { keyErr = true; pk = Bytes(48, 0); }
+        const uint8_t st = verifyStatus({pk}, {v.Payload}, {message_})[0];
+        if (keyErr || st == HBLS_VB_BAD_KEY_ENCODING) return errKeyDeserialize;
+        for (auto& k : v.SenderPubkeys) if (BallotBox.count(k)) return errAlreadyReceived;
+        if (st == HBLS_VB_BAD_SIG_ENCODING) return errSigDeserialize;
+        if (st != HBLS_VB_OK) return errVoteSig;
+        for (size_t a = 0; a < v.SenderPubkeys.size(); a++) for (size_t b = a + 1; b < v.SenderPubkeys.size(); b++)
+            if (v.SenderPubkeys[a] == v.SenderPubkeys[b]) return errDuplicateKey;
+        for (auto& k : v.SenderPubkeys) BallotBox[k] = Ballot{v.SenderPubkeys, v.Payload};
+        bool member = true; for (auto& k : v.SenderPubkeys) member &= index_.count(k) != 0;
+        Bytes bm(blen_, 0);
+        if (member) for (auto& k : v.SenderPubkeys) { const size_t x = index_.at(k); bm[x >> 3] |= (uint8_t)(1u << (x & 7)); }
+        else for (auto& k : v.SenderPubkeys) unbitted_.insert(k);
+        if (box_.AddVote(bm, v.Payload) < 0) throw std::runtime_error("hbls_ballot_box_add_vote failed");
+        for (size_t x = 0; x < blen_; x++) bitmap[x] |= bm[x];
+        return member ? "" : errKeyNotFound;
+    }
+};
 }  // namespace consensus
 
 namespace slash {      // == staking/slash/double-sign.go:139-168,215-262, the ballot checks that need no chain state

@@ -252,6 +252,39 @@ public:
     size_t BitmapLen() const { return (n_ + 7) >> 3; }
     const hbls_committee* handle() const { return h_; }
 };
+// running vote aggregate over a device-resident committee (hbls_ballot_box_*): the collected bitmap and the G2 sum of the collected
+// signatures; each signature is decoded once, when its vote arrives (quorum.go:164-196 AggregateVotes re-decodes every ballot)
+class BallotBox {
+    hbls_ballot_box* h_ = nullptr; size_t blen_ = 0;
+public:
+    BallotBox() = default;
+    BallotBox(const BallotBox&) = delete; BallotBox& operator=(const BallotBox&) = delete;
+    ~BallotBox() { if (h_) hbls_ballot_box_destroy(h_); }
+    std::string Create(const Committee& c) {
+        if (h_) { hbls_ballot_box_destroy(h_); h_ = nullptr; }
+        if (hbls_ballot_box_create(&h_, c.handle()) != 0) return "hbls_ballot_box_create failed";
+        blen_ = c.BitmapLen(); return "";
+    }
+    size_t BitmapLen() const { return blen_; }
+    // one ballot: 0 added, 1 skipped (a signer is already collected), HBLS_ERR_DECODE for an undecodable signature, < 0 error
+    int AddVote(const std::vector<uint8_t>& signerBitmap, const std::vector<uint8_t>& sig96) {
+        if (signerBitmap.size() != blen_ || sig96.size() != BLSSignatureSizeInBytes) return HBLS_ERR_ARG;
+        return hbls_ballot_box_add_vote(h_, signerBitmap.data(), blen_, sig96.data());
+    }
+    // a leader's queue of k votes on msg (bitmaps: k * BitmapLen() bytes, sigs: 96 k): status[j] = HBLS_BALLOT_*; "" or the error
+    std::string SubmitVotes(const std::vector<uint8_t>& bitmaps, const std::vector<uint8_t>& sigs, const std::vector<uint8_t>& msg, std::vector<uint8_t>& status) {
+        const size_t k = sigs.size() / 96;
+        if (sigs.size() != 96 * k || bitmaps.size() != k * blen_) return "vote queue: bitmap / signature sizes do not match";
+        status.assign(k, 0);
+        const int rc = hbls_ballot_box_submit_votes(h_, k, bitmaps.data(), blen_, sigs.data(), msg.data(), msg.size(), status.data());
+        return rc == 0 ? "" : rc == HBLS_ERR_ARG ? "hbls_ballot_box_submit_votes: bad argument" : "hbls_ballot_box_submit_votes failed";
+    }
+    // aggregate signature of the collected ballots and their bitmap (construct.go:158-175)
+    bool Aggregate(std::vector<uint8_t>& sig96, std::vector<uint8_t>& bitmap) const {
+        sig96.assign(96, 0); bitmap.assign(blen_, 0);
+        return hbls_ballot_box_aggregate(h_, sig96.data(), bitmap.data(), blen_) == 0;
+    }
+};
 // batch entry points test large batches in random-linear-combination groups first (exact fallback); exactOnly forces the per-round algorithm
 inline void SetBatchMode(bool exactOnly) { hbls_set_batch_mode(exactOnly ? 0 : 1); }
 // == NewMask(pubKeys).SetMask(bitmap) ; aggSig.Deserialize ; aggSig.VerifyHash(mask.AggregatePublic, msg)

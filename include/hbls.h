@@ -126,7 +126,8 @@ int hbls_aggregate_verify_batch(const hbls_committee* c, size_t B, const uint8_t
  * mode 0: the exact per-round check only (identical semantics to N calls of hbls_aggregate_verify). */
 void hbls_set_batch_mode(int mode);
 int  hbls_get_batch_mode(void);
-/* what the most recent batch call (aggregate_verify_batch[_device], verify_batch, aggregate_verify_items, verify_headers) did:
+/* what the most recent batch call (aggregate_verify_batch[_device], verify_batch, aggregate_verify_items, verify_headers,
+ * ballot_box_submit_votes) did:
  * waits for that call's device work if it is still running.  0 ok, HBLS_ERR_ARG if no batch call was made yet. */
 typedef struct {
     int32_t  mode;              /* 1: batched groups (+ exact pass over failed groups), 0: exact per round */
@@ -216,6 +217,26 @@ typedef struct hbls_ballot_box hbls_ballot_box;
 int  hbls_ballot_box_create(hbls_ballot_box** out, const hbls_committee* c);
 void hbls_ballot_box_destroy(hbls_ballot_box* b);
 int  hbls_ballot_box_add_vote(hbls_ballot_box* b, const uint8_t* signer_bitmap, size_t blen, const uint8_t sig96[96]);
+/* A leader's queue of k votes on one message (consensus/leader.go:110-345 onPrepare / onCommit) checked and collected in one call:
+ * vote j = (signer bitmap j over the box's committee, blen bytes each back to back ; signature j, sigs96 + 96 j), every vote on msg
+ * (msg_len <= 64).  The signers' keys come from the committee table, so no key is decoded; H(msg) is hashed once (H(m) cache).  The
+ * votes are judged in arrival order, in the order the reference meets the errors, and status[j] receives:
+ *   HBLS_BALLOT_COLLECTED          a signer is already collected: by a ballot in the box, or by a vote accepted earlier in this queue
+ *                                  (leader.go:227-235; decided before the signature is looked at)
+ *   HBLS_BALLOT_BAD_SIG_ENCODING   the signature does not decode (leader.go:254-257)
+ *   HBLS_BALLOT_BAD_SIG            VerifyHash(sum of the signer keys, msg) is false -- an empty bitmap included (identity key, above)
+ *   HBLS_BALLOT_ACCEPTED           the signers join the box's bitmap and the decoded signature its running sum
+ * Afterwards hbls_ballot_box_aggregate returns what AggregateVotes (quorum.go:164-196) gives over the accepted ballots, and
+ * hbls_ballot_box_add_vote keeps working on the same box.  Padding bits of the last bitmap byte are ignored.  The values differ from
+ * the HBLS_VB_* codes, so a status array cannot be read under the wrong table.  Committees of up to 16 384 slots.  0 ok (k == 0
+ * included), HBLS_ERR_ARG for a null box / status, blen != (n + 7) >> 3 or msg_len > 64.  Sets hbls_last_batch_info like the
+ * batch entries. */
+#define HBLS_BALLOT_ACCEPTED         16
+#define HBLS_BALLOT_COLLECTED        17
+#define HBLS_BALLOT_BAD_SIG_ENCODING 18
+#define HBLS_BALLOT_BAD_SIG          19
+int  hbls_ballot_box_submit_votes(hbls_ballot_box* b, size_t k, const uint8_t* signer_bitmaps, size_t blen,
+                                  const uint8_t* sigs96, const void* msg, size_t msg_len, uint8_t* status);
 /* aggregate signature of the collected votes + their bitmap (construct.go:158-175 constructQuorumSigAndBitmap) */
 int  hbls_ballot_box_aggregate(const hbls_ballot_box* b, uint8_t out_sig96[96], uint8_t* bitmap_out, size_t blen);
 
