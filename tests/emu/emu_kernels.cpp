@@ -319,3 +319,33 @@ extern "C" int emu_pair_decode_hash(size_t n, const uint8_t* sigs96, const uint8
     }
     return res;
 }
+
+// the decode kernels of every entry point on n serialized points (48 bytes for forms 0-2, 96 for forms 3-8): ok[i] = 1 decoded,
+// 0 rejected.  form 0 k_g1_decode, 1 k_g1_decode_jac, 2 k_single OP_G1_DES, 3 k_g2_decode, 4 k_g2_decode (no order check) +
+// k_g2_subgroup, 5 k_g2_decode_pair, 6 k_g2_decode_pair (no order check) + k_g2_subgroup_pair, 7 k_single OP_G2_DES, 8 k_single
+// OP_G2_DES_ADD.  check = 0 drops the subgroup test from forms 0, 1, 3 and 5 (the decode alone).  Returns 0, or -1 for an unknown form.
+extern "C" int emu_decode_flags(int form, int check, size_t n, const uint8_t* in, uint8_t* ok) {
+    std::vector<g1a> p1(n); std::vector<g1> j1(n); std::vector<g2a> p2(n); std::vector<g2> j2(n);
+    auto single = [&](int op, size_t w) {
+        std::vector<single_desc> d(n); std::vector<int> rc(n, -5);
+        for (size_t i = 0; i < n; i++) { pt_set_inf(j2[i]); d[i] = single_desc{in + w * i, nullptr, op == OP_G1_DES ? (void*)&j1[i] : (void*)&j2[i], op, 0u}; }
+        run_seq(1, (unsigned)n, [&] { k_single(n, d.data(), d[0], rc.data()); });
+        for (size_t i = 0; i < n; i++) ok[i] = rc[i] == (int)w ? 1 : 0;
+    };
+    switch (form) {
+    case 0: run_seq(1, (unsigned)n, [&] { k_g1_decode(n, in, p1.data(), ok, check, 0); }); break;
+    case 1: run_seq(1, (unsigned)n, [&] { k_g1_decode_jac(n, in, j1.data(), ok, check); }); break;
+    case 2: single(OP_G1_DES, 48); break;
+    case 3: run_seq(1, (unsigned)n, [&] { k_g2_decode(n, in, p2.data(), ok, check); }); break;
+    case 4: run_seq(1, (unsigned)n, [&] { k_g2_decode(n, in, p2.data(), ok, 0); });
+            run_seq(1, (unsigned)n, [&] { k_g2_subgroup(n, p2.data(), ok); }); break;
+    case 5: for (size_t i = 0; i < n; i++) run_pair([&] { k_g2_decode_pair(1, in + 96 * i, &p2[i], &ok[i], check); }); break;
+    case 6: { std::vector<uint8_t> dec(n);
+            for (size_t i = 0; i < n; i++) run_pair([&] { k_g2_decode_pair(1, in + 96 * i, &p2[i], &dec[i], 0); });
+            for (size_t i = 0; i < n; i++) run_pair([&] { k_g2_subgroup_pair(1, &p2[i], &dec[i], &ok[i]); }); break; }
+    case 7: single(OP_G2_DES, 96); break;
+    case 8: single(OP_G2_DES_ADD, 96); break;
+    default: return -1;
+    }
+    return 0;
+}
