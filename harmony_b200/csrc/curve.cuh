@@ -321,9 +321,9 @@ HB_DEV void rlc_scale_g1(g1& ra, const g1& apk, uint64_t c) {
     pt_mul_2d(ra, apk, p2, a, b);
 #endif
 }
-HB_DEV void rlc_scale_g2(g2& rs, const g2a& sig, uint64_t c) {
+template <class E> HB_DEV void rlc_scale_g2(jac<E>& rs, const aff<E>& sig, uint64_t c) {
     const uint32_t a = (uint32_t)c | 1u, b = (uint32_t)(c >> 32);
-    g2a q2;
+    aff<E> q2;
     fp2_mul_fp(q2.x, sig.x, fp_k(K_PSI2_CX)); fp2_neg(q2.y, sig.y);
 #if HB_JSF
     pt_mul_2d_aff_jsf(rs, sig, q2, a, b);

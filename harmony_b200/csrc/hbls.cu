@@ -43,7 +43,7 @@ struct Ctx {
     bool stage_timing = false; Scratch* stage_sc = nullptr;
     int batch_mode = 1;                                     // 1: random-linear-combination groups + exact pass over failed groups, 0: exact per round
     // tuning (hbls_set_param)
-    long long rlc_min = 12288, rlc_g = 0, tpsm = 384, tpsm_split = 512, tpsm_light = 1024, coop_max = 4096, overlap = 1, coop_wpsm = 14, hash_coop_max = 528, mask_sort = 1, hash_split = 2, tpsm_sw = 512, hash_fallback = 0, rlc_two_phase = 2, tpsm_lines = 512, tpsm_accum = 512, tpsm_cof = 512, tpsm_dec = 512, tpsm_scale = 384, tpsm_scale_g1 = 384, scale_split = 1, decode_split = 1, exact_two_phase = 1;
+    long long rlc_min = 12288, rlc_g = 0, tpsm = 384, tpsm_split = 512, tpsm_light = 1024, coop_max = 4096, overlap = 1, coop_wpsm = 14, hash_coop_max = 528, mask_sort = 1, hash_split = 2, tpsm_sw = 512, hash_fallback = 0, rlc_two_phase = 2, tpsm_lines = 512, tpsm_accum = 512, tpsm_cof = 512, tpsm_dec = 512, tpsm_sub = 512, tpsm_scale = 384, tpsm_scale_g2 = 512, tpsm_scale_g1 = 384, scale_split = 1, decode_split = 1, exact_two_phase = 1;
     int* rlc_form = nullptr;                                // device: 1 = the last call that could use blocks had many failed groups (k_rlc_form)
     long long rlc_block = 0;                                // blocks of HB_RLC_M groups (rlc_blocks): 0 automatic, 1 forced on, 2 forced off
     // coefficient stream: ChaCha20 keyed from /dev/urandom, block counter = call number
@@ -165,6 +165,8 @@ unsigned capped_blocks(size_t n, long long tpsm, unsigned tpb) {
 unsigned heavy_blocks(size_t n) { return capped_blocks(n, g.tpsm, TPB); }
 unsigned light_blocks(size_t n) { return capped_blocks(n, g.tpsm_light, TPB); }       // small-state kernels: the register count decides
 unsigned split_blocks(size_t nthreads) { return capped_blocks(nthreads, g.tpsm_split, HB_TPB_SPLIT); }
+// lock-stepped lane-pair kernels: one CTA per SM, its size = the resident threads wanted for that kernel (multiple of 64, <= 512)
+unsigned lockstep_cta(long long t) { t = t < 64 ? 64 : (t > HB_TPB_SPLIT ? HB_TPB_SPLIT : t); return (unsigned)(t & ~63ll); }
 
 // hash-to-G2 of a small batch (latency path): one WARP per message while that still leaves every warp its own scheduler's worth of
 // an SM (the cofactor clearing runs as VM step programs), else one message per lane pair
@@ -179,7 +181,8 @@ void launch_hash_batch(cudaStream_t s, size_t B, const uint8_t* d_msgs, uint32_t
     if (g.hash_split && HB_BATCH_INV) {
         LAUNCH(k_hash_sw, capped_blocks(B, g.tpsm_sw, TPB), TPB, s, B, d_msgs, msg_len, hm, ok_hm);
         if (g.hash_split >= 2) {        // three kernels: map | cofactor clearing (Jacobian, into the S buffer the scaling stage fills later) | affine
-            LAUNCH(k_hash_cofactor_jac, capped_blocks(B, g.tpsm_cof, TPB), TPB, s, B, (const g2a*)hm, (const uint8_t*)ok_hm, S);
+            const unsigned t = lockstep_cta(g.tpsm_cof);
+            LAUNCH(k_hash_cofactor_pair, capped_blocks(2 * B, t, t), t, s, B, (const g2a*)hm, (const uint8_t*)ok_hm, S);
             LAUNCH(k_g2_normalize_batch, heavy_blocks(B), TPB, s, B, (const g2*)S, hm);
         } else
             LAUNCH(k_hash_cofactor, heavy_blocks(B), TPB, s, B, hm, (const uint8_t*)ok_hm);
@@ -338,7 +341,8 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
     if (pairs) LAUNCH(k_g2_decode_pair, blocks_for(2 * B, 32), 32, sd, B, d_sig96, v.sig, v.ok_sig, warm ? 0 : 1);
     else if (g.decode_split) {
         LAUNCH(k_g2_decode, capped_blocks(B, g.tpsm_dec, TPB), TPB, s, B, d_sig96, v.sig, v.ok_sig, 0);
-        LAUNCH(k_g2_subgroup, capped_blocks(B, g.tpsm_dec, TPB), TPB, s, B, v.sig, v.ok_sig);
+        const unsigned t = lockstep_cta(g.tpsm_sub);
+        LAUNCH(k_g2_subgroup_pair, capped_blocks(2 * B, t, t), t, s, B, v.sig, (const uint8_t*)v.ok_sig, v.ok_sig, 1);
     } else LAUNCH(k_g2_decode, capped_blocks(B, g.tpsm_dec, TPB), TPB, s, B, d_sig96, v.sig, v.ok_sig, 1);
     if (warm) {
         cudaEventRecord(sc->mid, sd);
@@ -391,7 +395,8 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
         if (blocks) LAUNCH(k_rlc_form, 1, 32, s, ng, g.rlc_block == 1 ? 1 : 0, (const int*)g.rlc_form, v.counts + 2);
         if (g.scale_split && HB_BATCH_INV) {
             LAUNCH(k_rlc_scale_g1, capped_blocks(nr, g.tpsm_scale_g1, TPB), TPB, s, nr, ng, v.apk, co, v.pk_scaled, S, cb, blk_gate);
-            LAUNCH(k_rlc_scale_g2, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+            const unsigned t = lockstep_cta(g.tpsm_scale_g2);
+            LAUNCH(k_rlc_scale_g2_pair, capped_blocks(2 * nr, t, t), t, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
         } else
         LAUNCH(k_rlc_scale, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, (const uint64_t*)nullptr, v.pk_scaled, v.S, v.bad, S, cb, blk_gate);
         if (G == 8) LAUNCH(k_rlc_group_sum<8>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
@@ -401,10 +406,8 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
             // running points in their own kernel (lines to HBM, read once), accumulator + final exponentiation in the second
             for (size_t g0 = 0; g0 < ng; g0 += rlc_chunk_groups()) {
                 const size_t ngc = ng - g0 < rlc_chunk_groups() ? ng - g0 : rlc_chunk_groups();
-                // one lock-stepped CTA per SM, its size = the resident threads wanted for that kernel (multiple of 64, <= 512)
-                auto cta = [](long long t) { t = t < 64 ? 64 : (t > HB_TPB_SPLIT ? HB_TPB_SPLIT : t); return (unsigned)(t & ~63ll); };
                 // a batch that does not fill the chip: 64-thread CTAs spread over the SMs (the line kernel has G + 1 times the lane pairs)
-                const unsigned lt = full ? cta(g.tpsm_lines) : 64, at = full ? cta(g.tpsm_accum) : 64;
+                const unsigned lt = full ? lockstep_cta(g.tpsm_lines) : 64, at = full ? lockstep_cta(g.tpsm_accum) : 64;
                 const unsigned lb = full ? capped_blocks(2 * (G + 1) * ngc, lt, lt) : blocks_for(2 * (G + 1) * ngc, 64);
                 const unsigned ab = full ? capped_blocks(2 * ngc, at, at) : blocks_for(2 * ngc, 64);
                 // blocks possible (one chunk): both forms are launched and the device gates (k_rlc_form) let exactly one of them run
@@ -910,12 +913,12 @@ int hbls_init_device(int device) {
         CK(cudaEventCreateWithFlags(&g.hm[i].filled, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&g.hm[i].read_done, cudaEventDisableTiming));
     }
     g.hm_cache = envll("HBLS_HM_CACHE", 1); g.mask_sort = envll("HBLS_MASK_SORT", 1); g.hash_coop_max = envll("HBLS_HASH_COOP_MAX", 4ll * g.sm_count);     // one warp per message while every scheduler gets one
-    g.rlc_two_phase = envll("HBLS_RLC_2P", 2); g.tpsm_lines = envll("HBLS_TPSM_LINES", 512); g.tpsm_accum = envll("HBLS_TPSM_ACCUM", 512); g.tpsm_cof = envll("HBLS_TPSM_COF", 512); g.tpsm_dec = envll("HBLS_TPSM_DEC", 512); g.tpsm_scale = envll("HBLS_TPSM_SCALE", 384); g.tpsm_scale_g1 = envll("HBLS_TPSM_SCALE_G1", 384); g.scale_split = envll("HBLS_SCALE_SPLIT", 1); g.decode_split = envll("HBLS_DECODE_SPLIT", 1); g.exact_two_phase = envll("HBLS_EXACT_2P", 1);
+    g.rlc_two_phase = envll("HBLS_RLC_2P", 2); g.tpsm_lines = envll("HBLS_TPSM_LINES", 512); g.tpsm_accum = envll("HBLS_TPSM_ACCUM", 512); g.tpsm_cof = envll("HBLS_TPSM_COF", 512); g.tpsm_dec = envll("HBLS_TPSM_DEC", 512); g.tpsm_sub = envll("HBLS_TPSM_SUB", 512); g.tpsm_scale = envll("HBLS_TPSM_SCALE", 384); g.tpsm_scale_g1 = envll("HBLS_TPSM_SCALE_G1", 384); g.tpsm_scale_g2 = envll("HBLS_TPSM_SCALE_G2", 512); g.scale_split = envll("HBLS_SCALE_SPLIT", 1); g.decode_split = envll("HBLS_DECODE_SPLIT", 1); g.exact_two_phase = envll("HBLS_EXACT_2P", 1);
     g.rlc_block = envll("HBLS_RLC_BLOCK", 0);
     g.hash_split = envll("HBLS_HASH_SPLIT", 2); g.tpsm_sw = envll("HBLS_TPSM_SW", 512);
     CK(cudaFuncSetAttribute(k_hash_sw, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_hash_cofactor, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
-    CK(cudaFuncSetAttribute(k_hash_cofactor_jac, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
+    CK(cudaFuncSetAttribute(k_hash_cofactor_pair, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_g2_normalize_batch, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     g.ready = true;
     return self_test_at_init();
@@ -935,7 +938,7 @@ struct ParamDef { const char* name; long long Ctx::* slot; };
 const ParamDef PARAMS[] = {
     {"rlc_min", &Ctx::rlc_min}, {"rlc_g", &Ctx::rlc_g}, {"tpsm", &Ctx::tpsm}, {"tpsm_split", &Ctx::tpsm_split}, {"tpsm_light", &Ctx::tpsm_light}, {"coop_max", &Ctx::coop_max},
     {"overlap", &Ctx::overlap}, {"coop_wpsm", &Ctx::coop_wpsm}, {"hm_cache", &Ctx::hm_cache}, {"hash_coop_max", &Ctx::hash_coop_max}, {"mask_sort", &Ctx::mask_sort}, {"hash_split", &Ctx::hash_split},
-    {"hash_fallback", &Ctx::hash_fallback}, {"rlc_two_phase", &Ctx::rlc_two_phase}, {"tpsm_cof", &Ctx::tpsm_cof}, {"tpsm_dec", &Ctx::tpsm_dec}, {"tpsm_scale", &Ctx::tpsm_scale}, {"tpsm_scale_g1", &Ctx::tpsm_scale_g1},
+    {"hash_fallback", &Ctx::hash_fallback}, {"rlc_two_phase", &Ctx::rlc_two_phase}, {"tpsm_cof", &Ctx::tpsm_cof}, {"tpsm_dec", &Ctx::tpsm_dec}, {"tpsm_sub", &Ctx::tpsm_sub}, {"tpsm_scale", &Ctx::tpsm_scale}, {"tpsm_scale_g1", &Ctx::tpsm_scale_g1}, {"tpsm_scale_g2", &Ctx::tpsm_scale_g2},
     {"scale_split", &Ctx::scale_split}, {"decode_split", &Ctx::decode_split}, {"exact_two_phase", &Ctx::exact_two_phase}, {"tpsm_lines", &Ctx::tpsm_lines}, {"tpsm_accum", &Ctx::tpsm_accum}, {"tpsm_sw", &Ctx::tpsm_sw},
     {"rlc_block", &Ctx::rlc_block}, {"selftest_flip", &Ctx::selftest_flip}};
 static long long* param_slot(const char* name) {

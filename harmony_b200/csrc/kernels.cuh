@@ -59,8 +59,8 @@ __global__ void __launch_bounds__(64, HB_DEC_MINBLOCKS) k_g2_decode(size_t n, co
   }
 }
 
-// subgroup test of already-decoded affine points, one per thread (second half of k_g2_decode when the stage runs as two kernels,
-// hbls.cu "decode_split": square-root chains | G2 ladder); a point outside the subgroup loses its ok flag and is zeroed
+// subgroup test of already-decoded affine points, one per thread; a point outside the subgroup loses its ok flag and is zeroed.  The
+// split decode stage (hbls.cu "decode_split") runs k_g2_subgroup_pair instead; this form is the reference tests compare it with.
 __global__ void __launch_bounds__(64, HB_DEC_MINBLOCKS) k_g2_subgroup(size_t n, g2a* pts, uint8_t* ok) {
   for (size_t i = HB_TID; i < n; i += HB_STRIDE) {
     if (!ok[i]) continue;
@@ -370,7 +370,8 @@ __global__ void __launch_bounds__(64, HB_SW_MINBLOCKS) k_hash_sw(size_t n, const
   }
 }
 // cofactor clearing alone, Jacobian result (no per-thread arrays of pending items: the frame is the group law's own temporaries), and
-// the shared-inversion affine conversion as its own small kernel
+// the shared-inversion affine conversion as its own small kernel.  hbls.cu runs the cofactor clearing as k_hash_cofactor_pair; this
+// one-thread form is the reference tests compare it with.
 __global__ void k_hash_cofactor_jac(size_t n, const g2a* pts, const uint8_t* ok, g2* out) {
   for (size_t i = HB_TID; i < n; i += HB_STRIDE) {
     g2 h; pt_set_inf(h);
@@ -756,16 +757,51 @@ __global__ void __launch_bounds__(32) k_fe2_coop(size_t B, const fp2* f1, const 
         __syncwarp();
     }
 }
-// subgroup test of already-decoded affine signatures, one item per lane pair (the second half of k_g2_decode_pair)
-__global__ void k_g2_subgroup_pair(size_t n, const g2a* pts, const uint8_t* ok_in, uint8_t* ok_out) {
-    const size_t i = HB_TID >> 1; if (i >= n) return;
-    const g2a a = pts[i];
-    bool good = ok_in[i] != 0;
-    if (good && !aff_is_inf(a)) {
-        jac<fp2h> q; fp2h_pack(q.x, a.x); fp2h_pack(q.y, a.y); fp2_one(q.z);
-        good = g2_in_subgroup(q);
+// ---- large-batch G2 ladders on the lane-pair carrier: one item per lane pair, persistent, one lock-stepped CTA per SM (hbls.cu
+// lockstep_cta).  The carrier halves each thread's state (frames of ~1.3 KB instead of 3-4.7 KB for one item per thread), so the
+// ladders' operands stay in L1 at 512 resident threads; the Fp-level work is the same.  Sweep `it` gives lane pair q item
+// it * pairs + q; a warp leaves as a whole once its first item is past n, and a CTA barrier per sweep keeps the warps of a CTA on
+// the same instruction-cache lines.
+template <class Body> HB_DEV void pair_sweep(size_t n, Body body) {
+    const size_t ppg = HB_STRIDE >> 1;
+    for (size_t it = 0; ; it++) {
+        if (it * ppg + ((HB_TID & ~(size_t)31) >> 1) >= n) break;
+        hb_lockstep<fp2h>();
+        const size_t i = it * ppg + (HB_TID >> 1);
+        if (i < n) body(i);
     }
-    if ((threadIdx.x & 1) == 0) ok_out[i] = good ? 1 : 0;
+}
+// subgroup test of already-decoded affine signatures (the second half of k_g2_decode_pair; for large batches the second half of the
+// split decode stage).  zero_bad: a point outside the subgroup is also zeroed in place, as k_g2_subgroup does.
+__global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_g2_subgroup_pair(size_t n, g2a* pts, const uint8_t* ok_in, uint8_t* ok_out,
+                                                                                      int zero_bad = 0) {
+    const int role = threadIdx.x & 1;
+    pair_sweep(n, [&](size_t i) {
+        const fp* a4 = reinterpret_cast<const fp*>(&pts[i]);
+        aff<fp2h> a; a.x.c = a4[role]; a.y.c = a4[2 + role];
+        const bool in = ok_in[i] != 0;
+        bool good = in;
+        if (good && !aff_is_inf(a)) {
+            jac<fp2h> q; q.x = a.x; q.y = a.y; fp2_one(q.z);
+            good = g2_in_subgroup(q);
+        }
+        if (zero_bad && in && !good) { fp* o = reinterpret_cast<fp*>(&pts[i]); fp_zero(o[role]); fp_zero(o[2 + role]); }
+        if (role == 0) ok_out[i] = good ? 1 : 0;
+    });
+}
+// cofactor clearing of the SW map's output (k_hash_sw) into the Jacobian buffer k_g2_normalize_batch converts: k_hash_cofactor_jac
+// on the lane-pair carrier
+__global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_hash_cofactor_pair(size_t n, const g2a* pts, const uint8_t* ok, g2* out) {
+    const int role = threadIdx.x & 1;
+    pair_sweep(n, [&](size_t i) {
+        jac<fp2h> h; pt_set_inf(h);
+        if (ok[i]) {
+            const fp* p4 = reinterpret_cast<const fp*>(&pts[i]);
+            jac<fp2h> a; a.x.c = p4[role]; a.y.c = p4[2 + role]; fp2_one(a.z);
+            g2_clear_cofactor(h, a);
+        }
+        fp* o = reinterpret_cast<fp*>(&out[i]); o[role] = h.x.c; o[2 + role] = h.y.c; o[4 + role] = h.z.c;
+    });
 }
 __global__ void __launch_bounds__(32) k_pairing_coop2(size_t B, const fp2* f1, const uint8_t* irr1, const g1a* pk_neg, const g2a* hm,
                                   const uint8_t* ok_a, const uint8_t* ok_b, const uint8_t* ok_c, uint8_t* results) {
@@ -912,6 +948,7 @@ __global__ void k_rlc_scale_g1(size_t B, size_t ng, const g1* apk, rlc_coeffs co
 #ifndef HB_SCALE_G2_MINBLOCKS
 #define HB_SCALE_G2_MINBLOCKS 1
 #endif
+// the G2 ladder of the stage, one round per thread: the reference for k_rlc_scale_g2_pair, which hbls.cu runs
 __global__ void __launch_bounds__(64, HB_SCALE_G2_MINBLOCKS) k_rlc_scale_g2(size_t B, size_t ng, const g1* apk, const g2a* sig, const g2a* hm, const uint8_t* ok_sig, const uint8_t* ok_hm,
                                const uint8_t* ok_pk, rlc_coeffs co, g2* S, uint8_t* bad, size_t blk_stride = 0, rlc_block_coeffs cb = {},
                                const unsigned* blk_gate = nullptr) {
@@ -924,6 +961,25 @@ __global__ void __launch_bounds__(64, HB_SCALE_G2_MINBLOCKS) k_rlc_scale_g2(size
     if (r == 1ull) pt_from_aff(rs, sg); else rlc_scale_g2(rs, sg, r);
     S[j] = rs; bad[j] = b ? 1 : 0;
   }
+}
+// k_rlc_scale_g2 on the lane-pair carrier (pair_sweep).  A warp's 16 pairs hold 16 consecutive rounds, which share their coefficient
+// (the 32 of a warp of the thread kernel do), so the JSF digits stay warp-uniform.
+__global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_scale_g2_pair(size_t B, size_t ng, const g1* apk, const g2a* sig, const g2a* hm,
+                               const uint8_t* ok_sig, const uint8_t* ok_hm, const uint8_t* ok_pk, rlc_coeffs co, g2* S, uint8_t* bad,
+                               size_t blk_stride = 0, rlc_block_coeffs cb = {}, const unsigned* blk_gate = nullptr) {
+  if (blk_gate && *blk_gate == 0) blk_stride = 0;
+  const int role = threadIdx.x & 1;
+  pair_sweep(B, [&](size_t j) {
+    const fp* s4 = reinterpret_cast<const fp*>(&sig[j]);
+    const fp* h4 = reinterpret_cast<const fp*>(&hm[j]);
+    aff<fp2h> sg, h; sg.x.c = s4[role]; sg.y.c = s4[2 + role]; h.x.c = h4[role]; h.y.c = h4[2 + role];
+    const bool b = !ok_sig[j] || !ok_hm[j] || (ok_pk && !ok_pk[j]) || fp_is_zero(apk[j].z) || aff_is_inf(sg) || aff_is_inf(h);
+    jac<fp2h> rs;
+    const uint64_t r = rlc_coeff(co, j, ng, blk_stride, cb);
+    if (r == 1ull) pt_from_aff(rs, sg); else rlc_scale_g2(rs, sg, r);
+    fp* o = reinterpret_cast<fp*>(&S[j]); o[role] = rs.x.c; o[2 + role] = rs.y.c; o[4 + role] = rs.z.c;
+    if (role == 0) bad[j] = b ? 1 : 0;
+  });
 }
 // per group: affine sum of its S_j
 template <int G> __global__ void k_rlc_group_sum(size_t ngroups, const g2* S, g2a* Sg) {

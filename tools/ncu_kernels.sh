@@ -13,11 +13,11 @@ ONLY="$*"
 cap k_rlc_accum_split 'k_rlc_accum_split' 270336
 cap k_rlc_lines_split 'k_rlc_lines_split' 270336
 cap k_hash_sw '^k_hash_sw$' 270336
-cap k_hash_cofactor_jac '^k_hash_cofactor_jac$' 270336
+cap k_hash_cofactor_pair '^k_hash_cofactor_pair$' 270336
 cap k_g2_decode '^k_g2_decode$' 270336
-cap k_g2_subgroup '^k_g2_subgroup$' 270336
+cap k_g2_subgroup_pair '^k_g2_subgroup_pair$' 270336
 cap k_rlc_scale_g1 '^k_rlc_scale_g1$' 270336
-cap k_rlc_scale_g2 '^k_rlc_scale_g2$' 270336
+cap k_rlc_scale_g2_pair '^k_rlc_scale_g2_pair$' 270336
 cap k_mask_aggregate_serial 'k_mask_aggregate_serial' 270336
 # latency path: ONE round (a warp per kernel)
 export HBLS_HM_CACHE=0
