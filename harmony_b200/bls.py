@@ -95,6 +95,7 @@ def lib():
         sig("hbls_fp_mul_batch", c.c_int, sz, vp, vp, vp)
         sig("hbls_kernel_launch_count", c.c_uint64)
         sig("hbls_build_info", c.c_int)
+        sig("hbls_get_device", c.c_int)
         sig("hbls_probe_mac32_per_s", c.c_double, c.c_int, c.POINTER(c.c_double))
         sig("hbls_get_address", c.c_int, c.POINTER(_Pub), vp)
         sig("hbls_last_error", c.c_int, vp, sz)
@@ -103,6 +104,9 @@ def lib():
         sig("hbls_get_param", c.c_longlong, u8p)
         sig("hbls_aggregate_verify_items", c.c_int, sz, c.POINTER(vp), vp, vp, vp, sz, vp)
         sig("hbls_verify_headers", c.c_int, vp, sz, vp, vp, sz, vp, sz, sz, vp)
+        sig("hbls_verify_batch_status_device", c.c_int, sz, vp, vp, vp, sz, vp, vp)
+        sig("hbls_verify_headers_device", c.c_int, vp, sz, vp, vp, sz, vp, sz, sz, vp, vp)
+        sig("hbls_aggregate_verify_items_device", c.c_int, sz, c.POINTER(vp), vp, vp, vp, sz, vp, vp)
         sig("hbls_rlc_partial", c.c_int, sz, vp, vp, vp, sz, vp)
         sig("hbls_rlc_fold", c.c_int, sz, vp)
         sig("hbls_mask_create", c.c_int, c.POINTER(vp), vp)
@@ -298,6 +302,20 @@ class Committee:
         if rc != 0: raise HblsError(f"hbls_verify_headers rc={rc}")
         return st.raw[:n]
 
+    def VerifyHeadersDevice(self, sigs, bitmaps, payloads, quorum: int, stream=None):
+        """hbls_verify_headers_device on uint8 CUDA tensors sigs [n,96], bitmaps [n,blen], payloads [n,payload_len]: a new uint8
+        tensor [n] of HDR_* codes, filled asynchronously on `stream` (default: torch.cuda.current_stream())."""
+        L = _need()
+        n = _rows(sigs, "sigs", 96)
+        _rows(bitmaps, "bitmaps", self.blen(), n)
+        payload_len = _rows_any(payloads, "payloads", n)
+        st, out, h = _device_call(stream, n, (sigs, bitmaps, payloads))
+        if n == 0: return out                # as VerifyHeaders: an empty range has no statuses (the C call would see a NULL output)
+        rc = L.hbls_verify_headers_device(self.h, n, _ptr(sigs), _ptr(bitmaps), self.blen(), _ptr(payloads), payload_len, int(quorum),
+                                          _ptr(out), h)
+        if rc != 0: raise HblsError(f"hbls_verify_headers_device rc={rc}")
+        return out
+
 HDR_BAD_SIG, HDR_OK, HDR_NO_QUORUM, HDR_BAD_ENCODING = 0, 1, 2, 3
 
 def AggregateVerifyItems(committees, bitmaps, sigs96: bytes, msgs: bytes, msg_len: int) -> bytes:
@@ -342,6 +360,83 @@ def VerifyBatchStatus(pks48: bytes, sigs96: bytes, msgs: bytes, msg_len: int) ->
     rc = _need().hbls_verify_batch_status(k, _buf(pks48), _buf(sigs96), _buf(msgs), msg_len, st)
     if rc != 0: raise HblsError(f"hbls_verify_batch_status rc={rc}")
     return st.raw[:k]
+
+# ---- device forms: inputs are uint8 CUDA tensors already on the library's device, the result is a new uint8 CUDA tensor filled
+# asynchronously on `stream` (default torch.cuda.current_stream()).  Inputs produced on another stream must be ordered before
+# `stream` by the caller.  torch is imported here only, so the ctypes layer above works without it.
+def _library_device():
+    d = int(_need().hbls_get_device())
+    if d < 0: raise HblsError(f"hbls_get_device rc={d}")
+    return d
+
+def _check_tensor(t, name):
+    import torch
+    dev = _library_device()
+    if not isinstance(t, torch.Tensor): raise HblsError(f"{name}: expected a torch.Tensor, got {type(t).__name__}")
+    if t.dtype != torch.uint8: raise HblsError(f"{name}: dtype {t.dtype}, expected torch.uint8")
+    if t.device != torch.device("cuda", dev): raise HblsError(f"{name}: on {t.device}, expected cuda:{dev}")
+    if not t.is_contiguous(): raise HblsError(f"{name}: not contiguous")
+
+def _rows(t, name, width, rows=None):
+    """t must be [rows, width]; -> rows"""
+    _check_tensor(t, name)
+    if t.dim() != 2 or t.shape[1] != width or (rows is not None and t.shape[0] != rows):
+        raise HblsError(f"{name}: shape {tuple(t.shape)}, expected [{'k' if rows is None else rows}, {width}]")
+    return int(t.shape[0])
+
+def _rows_any(t, name, rows):
+    """t must be [rows, width] for some width; -> width"""
+    _check_tensor(t, name)
+    if t.dim() != 2 or t.shape[0] != rows: raise HblsError(f"{name}: shape {tuple(t.shape)}, expected [{rows}, len]")
+    return int(t.shape[1])
+
+def _ptr(t): return ctypes.c_void_p(t.data_ptr())
+
+_CUDA_STREAM_LEGACY = 1         # cudaStreamLegacy: torch's default stream (handle 0); NULL would mean the library's own stream
+
+def _device_call(stream, k, inputs):
+    """-> (stream, new [k] uint8 output, stream handle for the C ABI).  The output comes from `stream`'s side of the caching
+    allocator (a block freed on another stream may still be read there); inputs used on a stream other than the current one are
+    kept alive for it."""
+    import torch
+    dev = torch.device("cuda", _library_device())
+    cur = torch.cuda.current_stream(dev)
+    st = cur if stream is None else stream
+    with torch.cuda.stream(st):
+        out = torch.empty(k, dtype=torch.uint8, device=dev)
+    if st != cur:
+        for t in inputs: t.record_stream(st)
+    return st, out, ctypes.c_void_p(st.cuda_stream or _CUDA_STREAM_LEGACY)
+
+def VerifyBatchStatusDevice(pks, sigs, msgs, stream=None):
+    """hbls_verify_batch_status_device: pks [k,48], sigs [k,96], msgs [k,msg_len] -> uint8 tensor [k] of VB_* codes."""
+    L = _need()
+    k = _rows(sigs, "sigs", 96)
+    _rows(pks, "pks", 48, k)
+    msg_len = _rows_any(msgs, "msgs", k)
+    st, out, h = _device_call(stream, k, (pks, sigs, msgs))
+    if k == 0: return out
+    rc = L.hbls_verify_batch_status_device(k, _ptr(pks), _ptr(sigs), _ptr(msgs), msg_len, _ptr(out), h)
+    if rc != 0: raise HblsError(f"hbls_verify_batch_status_device rc={rc}")
+    return out
+
+def AggregateVerifyItemsDevice(committees, bitmaps, sigs, msgs, stream=None):
+    """hbls_aggregate_verify_items_device: item j = (committees[j], its bitmap, sigs[j], msgs[j]) -> uint8 tensor [k] of 1 / 0.
+    bitmaps: [k, blen] when every committee has blen bitmap bytes, else the items' bitmaps back to back as a 1-D tensor."""
+    L = _need()
+    k = len(committees)
+    _rows(sigs, "sigs", 96, k)
+    msg_len = _rows_any(msgs, "msgs", k)
+    _check_tensor(bitmaps, "bitmaps")
+    total = sum(c.blen() for c in committees)
+    if bitmaps.numel() != total or bitmaps.dim() not in (1, 2) or (bitmaps.dim() == 2 and bitmaps.shape[0] != k):
+        raise HblsError(f"bitmaps: shape {tuple(bitmaps.shape)}, expected {total} bytes ([k, blen] or back to back)")
+    arr = (ctypes.c_void_p * max(k, 1))(*[c.h for c in committees])
+    st, out, h = _device_call(stream, k, (bitmaps, sigs, msgs))
+    if k == 0: return out
+    rc = L.hbls_aggregate_verify_items_device(k, arr, _ptr(bitmaps), _ptr(sigs), _ptr(msgs), msg_len, _ptr(out), h)
+    if rc != 0: raise HblsError(f"hbls_aggregate_verify_items_device rc={rc}")
+    return out
 
 PARTIAL_BYTES = 872
 def RlcPartial(pks48: bytes, sigs96: bytes, msgs: bytes, msg_len: int) -> bytes:

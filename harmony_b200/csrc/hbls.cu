@@ -16,6 +16,7 @@
 #include "../../include/hbls.h"
 #include "coalesce.hpp"
 #include "kernels.cuh"
+#include "device_forms.cuh"
 
 using namespace hb;
 
@@ -30,6 +31,9 @@ struct Scratch {
     cudaEvent_t done = nullptr;
     cudaEvent_t fork = nullptr, join[2] = {}; bool forked = false;      // small batches: decode / hash on two auxiliary streams
     cudaEvent_t mid = nullptr, join2 = nullptr;                          // H(m) cached: "signature decoded" / "subgroup test done"
+    // device items form: the mask_item descriptors built on the host, pinned; `items_copied` is recorded after their upload, and the
+    // next call on this stream waits for it before it rewrites the buffer
+    mask_item* h_items = nullptr; size_t h_items_cap = 0; cudaEvent_t items_copied = nullptr; bool items_pending = false;
 };
 struct Ctx {
     bool ready = false;
@@ -307,12 +311,49 @@ static bool exact_two_phase(size_t B) { return g.rlc_two_phase >= 2 && g.exact_t
 // exact check of n rounds (contiguous arrays) as "groups" of one round through k_rlc_lines_split<1> / k_rlc_accum_split<1>
 void launch_exact_two_phase(size_t n, const g2a* sig, const g1a* pkneg, const g2a* hm, const uint8_t* ok_a, const uint8_t* ok_b, const uint8_t* ok_c,
                             uint8_t* bad, uint8_t* verdict, fp* lines, uint8_t* d_results, cudaStream_t s);
+// Message grouping of the device forms (device_forms.cuh): a hash table of >= 2k slots, the distinct messages' keys and points
+struct MsgGroups { uint32_t mask; uint32_t* slot_item; uint32_t* slot_rep; uint32_t* item_slot; uint32_t* pos; uint32_t* grp; uint8_t* keys;
+                   unsigned* count; g2a* hm_d; uint8_t* ok_d; };
+size_t group_slots(size_t k) { size_t T = 64; while (T < 2 * k) T <<= 1; return T; }
+size_t group_bytes(size_t k) { return group_slots(k) * 8 + k * (12 + 48 + sizeof(g2a) + 1) + 10 * 256; }
+MsgGroups carve_groups(Arena& ar, size_t k) {
+    MsgGroups m; const size_t T = group_slots(k);
+    m.mask = (uint32_t)(T - 1); m.slot_item = ar.take<uint32_t>(T); m.slot_rep = ar.take<uint32_t>(T);
+    m.item_slot = ar.take<uint32_t>(k); m.pos = ar.take<uint32_t>(k); m.grp = ar.take<uint32_t>(k); m.keys = ar.take<uint8_t>(48 * k);
+    m.count = ar.take<unsigned>(1); m.hm_d = ar.take<g2a>(k); m.ok_d = ar.take<uint8_t>(k);
+    return m;
+}
+// H(m) of the k items through their d distinct messages: group, hash the d keys with the form d calls for (launch_hash_small /
+// launch_hash_batch with d in place of k: warp per message up to hash_coop_max, lane pair up to coop_max -- or k on the latency
+// path --, thread per message beyond), gather to hm / ok_hm.  `pairs`: the call is on the latency path (no thread-per-item form).
+void launch_hash_grouped(cudaStream_t s, size_t k, const MsgGroups& m, const uint8_t* d_msgs, uint32_t msg_len, bool pairs, g2a* hm,
+                         uint8_t* ok_hm, g2* S) {
+    cudaMemsetAsync(m.slot_item, 0xff, (size_t)(m.mask + 1) * 4, s);
+    cudaMemsetAsync(m.slot_rep, 0xff, (size_t)(m.mask + 1) * 4, s);
+    uint32_t blk[16]; chacha20_block(g.chacha_key, ++g.rlc_calls, blk);          // the table's hash key: fresh per call, never seen outside
+    const uint64_t k0 = ((uint64_t)blk[1] << 32) | blk[0], k1 = ((uint64_t)blk[3] << 32) | blk[2];
+    LAUNCH(k_group_insert, blocks_for(k, 256), 256, s, k, d_msgs, msg_len, m.mask, k0, k1, m.slot_item, m.slot_rep, m.item_slot);
+    LAUNCH(k_group_compact, 1, HB_GRP_SCAN, s, k, d_msgs, msg_len, (const uint32_t*)m.slot_rep, (const uint32_t*)m.item_slot, m.pos, m.grp, m.keys, m.count);
+    const unsigned long long coop_hi = (unsigned long long)g.hash_coop_max;
+    const unsigned long long pair_hi = pairs ? (unsigned long long)k : (unsigned long long)(g.coop_max > g.hash_coop_max ? g.coop_max : g.hash_coop_max);
+    if (!pairs) {          // map, then cofactor clearing and affine conversion over all k slots (the identity beyond what the map wrote)
+        LAUNCH(k_hash_keys_sw, capped_blocks(k, g.tpsm_sw, TPB), TPB, s, k, (const unsigned*)m.count, pair_hi, (const uint8_t*)m.keys, m.hm_d, m.ok_d);
+        const unsigned t = lockstep_cta(g.tpsm_cof);
+        LAUNCH(k_hash_cofactor_pair, capped_blocks(2 * k, t, t), t, s, k, (const g2a*)m.hm_d, (const uint8_t*)m.ok_d, S);
+        LAUNCH(k_g2_normalize_batch, heavy_blocks(k), TPB, s, k, (const g2*)S, m.hm_d);
+    }
+    const size_t cg = (long long)k < g.hash_coop_max ? k : (size_t)(g.hash_coop_max > 0 ? g.hash_coop_max : 1);
+    LAUNCH(k_hash_keys_coop, (unsigned)cg, 32, s, (const unsigned*)m.count, coop_hi, (const uint8_t*)m.keys, m.hm_d, m.ok_d, (int)g.hash_fallback);
+    LAUNCH(k_hash_keys_pair, blocks_for(2 * k, 32), 32, s, (const unsigned*)m.count, coop_hi, pair_hi, (const uint8_t*)m.keys, m.hm_d, m.ok_d);
+    LAUNCH(k_broadcast_hm, blocks_for(k, 256), 256, s, k, (const uint32_t*)m.grp, (const g2a*)m.hm_d, (const uint8_t*)m.ok_d, hm, ok_hm);
+}
 #define STAGE_EV(i, sc, strm) do { if (g.stage_timing && (sc)->ev_ok) cudaEventRecord((sc)->ev[i], (strm)); } while (0)
 // v.apk holds the Jacobian (aggregate) public key of every round; ok_pk (nullable) = per-round "key decoded" flags of the triple form
 // h_msg (nullable): host copy of THE message when the call has a single one (one round, or a same-message batch) -- the key of the
-// H(m) cache
+// H(m) cache.  mg (nullable, device forms): H(m) once per distinct message, grouped on the device (same_msg / h_msg unused)
 void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_t* d_sig96, const uint8_t* d_msgs, uint32_t msg_len,
-                        const uint8_t* ok_pk, uint8_t* d_results, cudaStream_t s, bool same_msg, const uint8_t* h_msg = nullptr) {
+                        const uint8_t* ok_pk, uint8_t* d_results, cudaStream_t s, bool same_msg, const uint8_t* h_msg = nullptr,
+                        const MsgGroups* mg = nullptr) {
     STAGE_EV(1, sc, s);
     const bool rlc = rlc_applies(B);
     // the batched check consumes the Jacobian sums directly; -apk in affine form is then only needed for the rounds of failed groups
@@ -349,7 +390,9 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
         LAUNCH(k_miller_pq_coop, coop_grid, 32, sd, B, (const g1a*)nullptr, v.sig, v.ok_sig, v.f1, v.irr1);
     } else if (split_ml) LAUNCH(k_miller1_coop, coop_grid, 32, sd, B, v.sig, v.ok_sig, v.f1, v.irr1);
     STAGE_EV(3, sc, s);
-    if (one_msg) {
+    if (mg)
+        launch_hash_grouped(sh, B, *mg, d_msgs, msg_len, pairs, v.hm, v.ok_hm, v.S);
+    else if (one_msg) {
         if (!hit) {
             if (pairs) launch_hash_small(sh, 1, d_msgs, msg_len, v.hm, v.ok_hm);
             else LAUNCH(k_hash_to_g2, 1, TPB, sh, (size_t)1, d_msgs, msg_len, v.hm, v.ok_hm);
@@ -820,7 +863,7 @@ void launch_mask_serial(const hbls_committee* c, size_t B, const uint8_t* d_bitm
 // rounds against one committee, everything device-resident
 int agg_verify_device_locked(const hbls_committee* c, size_t B, const uint8_t* d_bitmaps, size_t blen, const uint8_t* d_sigs,
                              const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, Arena& ar, bool same_msg,
-                             VerifyBufs* v_out = nullptr, const uint8_t* h_msg = nullptr) {
+                             VerifyBufs* v_out = nullptr, const uint8_t* h_msg = nullptr, const MsgGroups* mg = nullptr) {
     VerifyBufs v = carve_verify(ar, B);
     fork_point(B, sc, s);
     STAGE_EV(0, sc, s);
@@ -828,7 +871,7 @@ int agg_verify_device_locked(const hbls_committee* c, size_t B, const uint8_t* d
         launch_mask_serial(c, B, d_bitmaps, blen, v, s);
     else
         LAUNCH(k_mask_aggregate, blocks_for(B * 32, 128), 128, s, B, c->n, c->table, d_bitmaps, blen, v.apk);
-    launch_verify_tail(B, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, same_msg, h_msg);
+    launch_verify_tail(B, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, same_msg, h_msg, mg);
     if (v_out) *v_out = v;
     return 0;
 }
@@ -931,6 +974,7 @@ int blsInit(int curve, int compiledTimeVar) {
 }
 uint64_t hbls_kernel_launch_count(void) { return g.launches.load(); }
 int hbls_build_info(void) { return (HB_BATCH_INV ? 1 : 0) | (HB_BATCH_K << 8); }
+int hbls_get_device(void) { if (int e = ensure_init()) return e; std::lock_guard<std::mutex> lk(g.mu); return g.device; }
 void hbls_set_batch_mode(int mode) { std::lock_guard<std::mutex> lk(g.mu); g.batch_mode = mode ? 1 : 0; }
 int hbls_get_batch_mode(void) { std::lock_guard<std::mutex> lk(g.mu); return g.batch_mode; }
 // tuning knobs by name (hbls_set_param); the self-test saves and restores all of them
@@ -1303,6 +1347,100 @@ int hbls_verify_batch_status(size_t k, const uint8_t* pk48, const uint8_t* sig96
     if (!status) return HBLS_ERR_ARG;
     std::lock_guard<std::mutex> lk(g.mu);
     return verify_batch_status_locked(k, pk48, sig96, msgs, msg_len, status);
+}
+
+// ------------------------------------------------------------------ device forms of the three batch verifiers above: inputs and
+// outputs in HBM (any byte alignment), everything enqueued on the caller's stream with no host synchronisation, statuses computed
+// on the device (device_forms.cuh), H(m) once per distinct message (grouped on the device; the H(m) cache is neither read nor
+// filled: the host never sees the messages).  Same kernels and batching regimes as the host forms otherwise.
+static int verify_batch_status_device_locked(size_t k, const uint8_t* d_pk, const uint8_t* d_sig, const uint8_t* d_msgs, size_t msg_len,
+                                             uint8_t* d_status, cudaStream_t s) {
+    Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(k) + group_bytes(k) + 2 * k + 4096, &sc)) return e;
+    ensure_stage_events(sc);
+    Arena ar{sc->base, 0, sc->cap};
+    VerifyBufs v = carve_verify(ar, k); const MsgGroups mg = carve_groups(ar, k);
+    uint8_t* dres = ar.take<uint8_t>(k); uint8_t* dflags = ar.take<uint8_t>(k);
+    fork_point(k, sc, s);
+    STAGE_EV(0, sc, s);
+    LAUNCH(k_g1_decode_jac, heavy_blocks(k), TPB, s, k, d_pk, v.apk, v.ok_pk, 1);
+    launch_verify_tail(k, v, sc, d_sig, d_msgs, (uint32_t)msg_len, v.ok_pk, dres, s, false, nullptr, &mg);
+    LAUNCH(k_pack_flags, blocks_for(k, 256), 256, s, k, v.ok_sig, v.ok_hm, (const uint8_t*)v.ok_pk, dflags);
+    LAUNCH(k_status_triples, blocks_for(k, 256), 256, s, k, (const uint8_t*)dflags, (const uint8_t*)dres, d_status);
+    CK(cudaGetLastError());
+    return 0;
+}
+int hbls_verify_batch_status_device(size_t k, const void* d_pk48, const void* d_sig96, const void* d_msgs, size_t msg_len, void* d_status, void* stream) {
+    if (int e = ensure_init()) return e;
+    if (k == 0) return 0;
+    if (!d_status) return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return verify_batch_status_device_locked(k, (const uint8_t*)d_pk48, (const uint8_t*)d_sig96, (const uint8_t*)d_msgs, msg_len, (uint8_t*)d_status,
+                                             stream ? (cudaStream_t)stream : g.stream);
+}
+static int verify_headers_device_locked(const hbls_committee* c, size_t n, const uint8_t* d_sigs, const uint8_t* d_bitmaps, size_t blen,
+                                        const uint8_t* d_payloads, size_t payload_len, size_t quorum, uint8_t* d_status, cudaStream_t s) {
+    Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(n) + group_bytes(n) + 2 * n + 4096, &sc)) return e;
+    ensure_stage_events(sc);
+    Arena ar{sc->base, 0, sc->cap};
+    const MsgGroups mg = carve_groups(ar, n);
+    uint8_t* dres = ar.take<uint8_t>(n); uint8_t* dflags = ar.take<uint8_t>(n);
+    VerifyBufs v;
+    agg_verify_device_locked(c, n, d_bitmaps, blen, d_sigs, d_payloads, payload_len, dres, s, sc, ar, false, &v, nullptr, &mg);
+    LAUNCH(k_pack_flags, blocks_for(n, 256), 256, s, n, v.ok_sig, v.ok_hm, (const uint8_t*)nullptr, dflags);
+    LAUNCH(k_status_headers, blocks_for(n, 256), 256, s, n, c->n, d_bitmaps, blen, quorum, (const uint8_t*)dflags, (const uint8_t*)dres, d_status);
+    CK(cudaGetLastError());
+    return 0;
+}
+int hbls_verify_headers_device(const hbls_committee* c, size_t n, const void* d_sigs96, const void* d_bitmaps, size_t blen,
+                               const void* d_payloads, size_t payload_len, size_t quorum, void* d_status, void* stream) {
+    if (int e = ensure_init()) return e;
+    if (!c || blen != ((c->n + 7) >> 3) || !d_status) return HBLS_ERR_ARG;
+    if (n == 0) return 0;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return verify_headers_device_locked(c, n, (const uint8_t*)d_sigs96, (const uint8_t*)d_bitmaps, blen, (const uint8_t*)d_payloads, payload_len, quorum,
+                                        (uint8_t*)d_status, stream ? (cudaStream_t)stream : g.stream);
+}
+// The descriptors (table, bitmap, slots per item) come from the host array of handles.  They are written into the stream's own pinned
+// buffer and uploaded with an asynchronous copy; an event recorded after that copy guards the buffer, so a later call on the same
+// stream waits (on the host) only if the earlier upload has not run yet.  A pageable copy would synchronise the stream.
+static int aggregate_verify_items_device_locked(size_t k, const hbls_committee* const* committees, const uint8_t* d_bitmaps, const uint8_t* d_sigs,
+                                                const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s) {
+    Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(k) + group_bytes(k) + k * sizeof(mask_item) + 4096, &sc)) return e;
+    ensure_stage_events(sc);
+    if (sc->items_pending) { CK(cudaEventSynchronize(sc->items_copied)); sc->items_pending = false; }
+    if (!sc->items_copied) CK(cudaEventCreateWithFlags(&sc->items_copied, cudaEventDisableTiming));
+    if (k > sc->h_items_cap) {
+        if (sc->h_items) CK(cudaFreeHost(sc->h_items));
+        sc->h_items = nullptr; sc->h_items_cap = 0;
+        CK(cudaMallocHost(&sc->h_items, k * sizeof(mask_item)));
+        sc->h_items_cap = k;
+    }
+    Arena ar{sc->base, 0, sc->cap};
+    VerifyBufs v = carve_verify(ar, k); const MsgGroups mg = carve_groups(ar, k);
+    mask_item* ditems = ar.take<mask_item>(k);
+    size_t off = 0;
+    for (size_t j = 0; j < k; j++) {
+        sc->h_items[j].table = committees[j]->table; sc->h_items[j].bitmap = d_bitmaps + off; sc->h_items[j].n = committees[j]->n;
+        off += (committees[j]->n + 7) >> 3;
+    }
+    CK(cudaMemcpyAsync(ditems, sc->h_items, k * sizeof(mask_item), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(sc->items_copied, s)); sc->items_pending = true;
+    fork_point(k, sc, s);
+    STAGE_EV(0, sc, s);
+    LAUNCH(k_mask_aggregate_items, blocks_for(k * 32, 128), 128, s, k, (const mask_item*)ditems, v.apk);
+    launch_verify_tail(k, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, false, nullptr, &mg);
+    CK(cudaGetLastError());
+    return 0;
+}
+int hbls_aggregate_verify_items_device(size_t k, const hbls_committee* const* committees, const void* d_bitmaps, const void* d_sigs96,
+                                       const void* d_msgs, size_t msg_len, void* d_results, void* stream) {
+    if (int e = ensure_init()) return e;
+    if (k == 0) return 0;
+    if (!committees || !d_results) return HBLS_ERR_ARG;
+    for (size_t j = 0; j < k; j++) if (!committees[j]) return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return aggregate_verify_items_device_locked(k, committees, (const uint8_t*)d_bitmaps, (const uint8_t*)d_sigs96, (const uint8_t*)d_msgs, msg_len,
+                                                (uint8_t*)d_results, stream ? (cudaStream_t)stream : g.stream);
 }
 
 // ------------------------------------------------------------------ persistent Mask / running vote aggregate (SURVEY 8f.2)

@@ -16,7 +16,7 @@
  * into shared device launches: while one turn runs on the GPU, or a batch call holds it, the calls that arrive queue up and the next
  * caller in line runs them all as one turn (hbls_coalesce_stats counts the turns).  There is no timer or batching window: a call
  * that finds the library idle runs at once, alone, with the launches it has always made.  Device work is serialised by one library
- * mutex and (except hbls_aggregate_verify_batch_device on a caller stream) one library stream.  Scratch memory is per stream, so
+ * mutex and (except the *_device entry points on a caller stream) one library stream.  Scratch memory is per stream, so
  * asynchronous device-pointer calls on DIFFERENT streams do not share intermediates; calls on one stream are stream-ordered.
  * Messages: only the first min(len, 48) bytes enter the map to G2 (mcl setArrayMask; SURVEY A.3); batch entry points take the
  * message stride msg_len and read min(msg_len, 48) bytes per item.
@@ -194,6 +194,24 @@ int hbls_aggregate_verify_items(size_t k, const hbls_committee* const* committee
 int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96, const uint8_t* bitmaps, size_t blen,
                         const uint8_t* payloads, size_t payload_len, size_t quorum, uint8_t* status);
 
+/* Device forms of hbls_verify_batch_status, hbls_verify_headers and hbls_aggregate_verify_items: every d_ pointer is device
+ * memory (HBM, any byte alignment), laid out as in the host form; committees stays a HOST array of handles.  stream = cudaStream_t
+ * or NULL (the library stream, which does NOT wait for the legacy default stream: a caller whose inputs come from work on the
+ * default stream passes cudaStreamLegacy).  The call enqueues its work on that stream and returns without waiting for the device: the
+ * statuses / results are in d_status / d_results once the stream reaches that point.  They are, byte for byte, what the host form
+ * writes for the same inputs (same codes in the same order of checks, same argument errors, same batching regimes), and the call
+ * sets hbls_last_batch_info.  Scratch is per stream, so calls on different streams can be in flight together.
+ * Messages: items whose messages agree in the 48 zero-padded bytes the map reads are grouped on the device and each distinct
+ * message is hashed to G2 once.  The H(m) cache is neither read nor filled (hbls_hash_cache_stats does not move).
+ * The first call on a stream, or one larger than any before it there, allocates scratch (which may wait for the device); the items
+ * form also waits, on the host, for the upload of the previous items call on the same stream if that has not run yet. */
+int hbls_verify_batch_status_device(size_t k, const void* d_pk48, const void* d_sig96, const void* d_msgs, size_t msg_len,
+                                    void* d_status, void* stream);
+int hbls_verify_headers_device(const hbls_committee* c, size_t n, const void* d_sigs96, const void* d_bitmaps, size_t blen,
+                               const void* d_payloads, size_t payload_len, size_t quorum, void* d_status, void* stream);
+int hbls_aggregate_verify_items_device(size_t k, const hbls_committee* const* committees, const void* d_bitmaps, const void* d_sigs96,
+                                       const void* d_msgs, size_t msg_len, void* d_results, void* stream);
+
 /* Persistent device Mask (SURVEY 8f.2; crypto/bls/mask.go:67-242; TODO(audit) at consensus/consensus_service.go:318): the
  * bitmap lives on the host, the running aggregate public key in HBM; SetMask / SetBit apply only the DELTA (Add on 0->1,
  * Sub on 1->0, mask.go:121-133,137-155) instead of rebuilding the sum.  Return 0 or HBLS_ERR_ARG (length / index). */
@@ -279,6 +297,9 @@ uint64_t hbls_kernel_launch_count(void);
 /* compile-time variant of the device code: bit 0 = shared inversions (Montgomery's trick over the items of a persistent thread in
  * hash-to-G2 and coefficient scaling), bits 8.. = items per shared inversion */
 int hbls_build_info(void);
+/* the CUDA device index the library was initialised on (device pointers of the *_device entry points live there), or the error of
+ * an uninitialised library */
+int hbls_get_device(void);
 /* device self-test of the lane-pair (split Fp2) primitives used by k_pairing_verify_split against the single-thread
  * primitives on pseudo-random operands: returns the number of mismatches (0 = pass), <0 on error */
 int hbls_selftest_split(uint32_t iters);
