@@ -1,11 +1,11 @@
 // harmony_b200/csrc/device_forms.cuh -- kernels of the device forms of the batch verifiers (include/hbls.h:
-// hbls_verify_batch_status_device, hbls_verify_headers_device, hbls_aggregate_verify_items_device).  Included by hbls.cu only.
-//
-// Their inputs never reach the host, so two things the host forms do on the CPU happen here:
-//   * message grouping: items whose messages agree in the 48 zero-padded bytes the map reads (hbls.cu hm_key) are one message;
-//     each distinct message is hashed to G2 once and the point gathered back to its items.  The representative of a group is its
-//     lowest item index (atomicMin), and the distinct messages are numbered in item order, so nothing depends on thread scheduling.
-//   * statuses: the HBLS_VB_* / HBLS_HDR_* codes from the k_pack_flags bits, in the order of checks of the host forms.
+// hbls_verify_batch_status_device, hbls_verify_headers_device, hbls_aggregate_verify_items_device), and the status kernels their
+// host forms share.  Included by hbls.cu only.
+//   * message grouping: the inputs of a device form never reach the host, so items whose messages agree in the 48 zero-padded bytes
+//     the map reads (hbls.cu hm_key) are found to be one message here; each distinct message is hashed to G2 once and the point
+//     gathered back to its items.  The representative of a group is its lowest item index (atomicMin), and the distinct messages
+//     are numbered in item order, so nothing depends on thread scheduling.
+//   * statuses: the HBLS_VB_* / HBLS_HDR_* codes from the k_pack_flags bits, the only place in the library they are assigned.
 #pragma once
 #include "../../include/hbls.h"
 #include "kernels.cuh"
@@ -91,8 +91,8 @@ __global__ void __launch_bounds__(HB_GRP_SCAN) k_group_compact(size_t k, const u
 
 // ---- hash-to-G2 of the d = *count distinct keys (48 bytes each).  d is known on the device only, so every form is launched and
 // runs only in its range of d: warp per message for d <= coop_hi, lane pair per message for coop_hi < d <= pair_hi, and the
-// thread-per-item map (then hbls.cu's cofactor / affine kernels over all k slots) for d > pair_hi.  Bodies as k_hash_to_g2_coop,
-// k_hash_to_g2_pair and k_hash_sw.
+// thread-per-item map (then hbls.cu's cofactor / affine kernels over all k slots) for d > pair_hi.  The per-item bodies are those of
+// k_hash_to_g2_coop, k_hash_to_g2_pair and k_hash_sw (kernels.cuh).
 __global__ void __launch_bounds__(32) k_hash_keys_coop(const unsigned* count, unsigned long long coop_hi, const uint8_t* keys, g2a* out,
                                                        uint8_t* ok, int force_fallback) {
     const size_t n = *count;
@@ -100,83 +100,34 @@ __global__ void __launch_bounds__(32) k_hash_keys_coop(const unsigned* count, un
     __shared__ uint32_t slots[VM_SMEM_WORDS];
     const int lane = threadIdx.x & 31;
     vm_load_consts(slots);
-    for (size_t i = blockIdx.x; i < n; i += gridDim.x) {
-        fp2 t; hash_to_fp(t.a, keys + (size_t)48 * i, 48); fp_zero(t.b);
-        g2 a; const bool good = sw_map_g2<true>(a, t);
-        g2a res; fp2_zero(res.x); fp2_zero(res.y);
-        if (good) {
-            if (lane == 0) { vm_set_fp2(slots, VM_R_Q2X, a.x); vm_set_fp2(slots, VM_R_Q2Y, a.y); }
-            __syncwarp();
-            if (vm_hash_cofactor(slots) && !force_fallback) {
-                if (lane == 0) { vm_ld(res.x.a.l, slots, VM_R_HX, 0); vm_ld(res.x.b.l, slots, VM_R_HX, 1); vm_ld(res.y.a.l, slots, VM_R_HY, 0); vm_ld(res.y.b.l, slots, VM_R_HY, 1); }
-            } else if (lane < 2) {
-                jac<fp2h> A, H; fp2h_pack(A.x, a.x); fp2h_pack(A.y, a.y); fp2h_pack(A.z, a.z);
-                g2_clear_cofactor(H, A);
-                if (!pt_is_inf(H)) {
-                    fp2h zi, zi2, hx, hy; fp2_inv_gcd(zi, H.z); fp2_sqr(zi2, zi);
-                    fp2_mul(hx, H.x, zi2); fp2_mul(zi2, zi2, zi); fp2_mul(hy, H.y, zi2);
-                    fp2h_unpack(res.x, hx); fp2h_unpack(res.y, hy);
-                }
-            }
-        }
-        if (lane == 0) { out[i] = res; ok[i] = good ? 1 : 0; }
-        __syncwarp();
-    }
+    for (size_t i = blockIdx.x; i < n; i += gridDim.x) HB_HASH_ITEM_WARP(i, keys, 48, out, ok, slots, lane, force_fallback)
 }
 __global__ void k_hash_keys_pair(const unsigned* count, unsigned long long coop_hi, unsigned long long pair_hi, const uint8_t* keys, g2a* out,
                                  uint8_t* ok) {
     const size_t n = *count, i = HB_TID >> 1;
     if (n <= coop_hi || n > pair_hi || i >= n) return;
-    fp2 t; hash_to_fp(t.a, keys + (size_t)48 * i, 48); fp_zero(t.b);
-    g2 a; bool good = sw_map_g2<true>(a, t);
-    g2a res; fp2_zero(res.x); fp2_zero(res.y);
-    if (good) {
-        jac<fp2h> A, H; fp2h_pack(A.x, a.x); fp2h_pack(A.y, a.y); fp2h_pack(A.z, a.z);
-        g2_clear_cofactor(H, A);
-        if (!pt_is_inf(H)) {
-            fp2h zi, zi2, hx, hy; fp2_inv_gcd(zi, H.z); fp2_sqr(zi2, zi);
-            fp2_mul(hx, H.x, zi2); fp2_mul(zi2, zi2, zi); fp2_mul(hy, H.y, zi2);
-            fp2h_unpack(res.x, hx); fp2h_unpack(res.y, hy);
-        }
-    }
-    if ((threadIdx.x & 1) == 0) { out[i] = res; ok[i] = good ? 1 : 0; }
+    HB_HASH_ITEM_PAIR(i, keys, 48, out, ok)
 }
 // writes all k slots: the map for i < d when d > pair_hi, else (and beyond d) the identity with ok = 0, so that the cofactor and
 // affine kernels that follow over k slots leave nothing the other forms have to undo
 __global__ void __launch_bounds__(64, HB_SW_MINBLOCKS) k_hash_keys_sw(size_t k, const unsigned* count, unsigned long long pair_hi,
                                                                       const uint8_t* keys, g2a* pts, uint8_t* ok) {
     const size_t d = *count, n = d > pair_hi ? d : 0;
-  for (size_t i0 = HB_TID; i0 < k; i0 += (size_t)HB_BATCH_K * HB_STRIDE) {
-    fp2 z[HB_BATCH_K], t[HB_BATCH_K], u[HB_BATCH_K], ct[HB_BATCH_K]; bool skip[HB_BATCH_K];
-    for (int j = 0; j < HB_BATCH_K; j++) {
-        const size_t i = i0 + (size_t)j * HB_STRIDE;
-        skip[j] = true;
-        if (i >= n) continue;
-        fp_zero(t[j].b); hash_to_fp(t[j].a, keys + (size_t)48 * i, 48);
-        skip[j] = !sw_map_g2_pre(u[j], ct[j], z[j], t[j]);
-    }
-    f_batch_inv<fp2, HB_BATCH_K>(z, skip);
-    for (int j = 0; j < HB_BATCH_K; j++) {
-        const size_t i = i0 + (size_t)j * HB_STRIDE;
-        if (i >= k) continue;
-        g2 a; g2a o; fp2_zero(o.x); fp2_zero(o.y);
-        const bool good = i < n && !skip[j] && sw_map_g2_post(a, t[j], u[j], ct[j], z[j]);
-        if (good) { o.x = a.x; o.y = a.y; }
-        pts[i] = o; ok[i] = good ? 1 : 0;
-    }
-  }
+    for (size_t i0 = HB_TID; i0 < k; i0 += (size_t)HB_BATCH_K * HB_STRIDE) hash_sw_items(i0, n, k, keys, 48, pts, ok);
 }
 
-// ---- statuses from the k_pack_flags bits (bit0 signature decoded, bit2 key decoded) and the verdicts
-// hbls_verify_batch_status: key decode first, then signature decode, then VerifyHash
+// ---- statuses from the k_pack_flags bits (bit0 signature decoded, bit2 key decoded) and the verdicts, for the host and device forms
+// alike, in the order the reference meets the errors.
+// hbls_verify_batch_status: key decode first (BytesToBLSPublicKey, consensus/view_change_msg.go:159), then signature decode
+// (Sign.Deserialize, :168-179), then VerifyHash
 __global__ void k_status_triples(size_t k, const uint8_t* flags, const uint8_t* results, uint8_t* status) {
     const size_t j = HB_TID; if (j >= k) return;
     const uint8_t f = flags[j];
     status[j] = !(f & 4) ? HBLS_VB_BAD_KEY_ENCODING : !(f & 1) ? HBLS_VB_BAD_SIG_ENCODING : results[j] == 1 ? HBLS_VB_OK : HBLS_VB_BAD_SIG;
 }
 HB_DEV uint32_t grp_popc8(uint32_t v) { v = v - ((v >> 1) & 0x55u); v = (v & 0x33u) + ((v >> 2) & 0x33u); return (v + (v >> 4)) & 0x0fu; }
-// hbls_verify_headers: signature decode, then the quorum over the committee's nslots slots (padding bits of the last byte never
-// count; quorum 0 skips the gate), then VerifyHash
+// hbls_verify_headers (engine.go:630-640): signature decode (DecodeSigBitmap), then the quorum over the committee's nslots slots
+// (IsQuorumAchievedByMask; padding bits of the last byte never count; quorum 0 skips the gate), then VerifyHash
 __global__ void k_status_headers(size_t n, size_t nslots, const uint8_t* bitmaps, size_t blen, size_t quorum, const uint8_t* flags,
                                  const uint8_t* results, uint8_t* status) {
     const size_t j = HB_TID; if (j >= n) return;

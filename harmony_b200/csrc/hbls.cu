@@ -1207,26 +1207,83 @@ int hbls_aggregate_verify_batch_device(const hbls_committee* c, size_t B, const 
     CK(cudaGetLastError());
     return rc;
 }
-// host-buffer form shared by the batch entry and the header-range entry: flags_out (nullable) receives the decode flags per round
+// ------------------------------------------------------------------ bodies of the batch verifiers, shared by their host and device
+// forms: inputs in HBM, work enqueued on stream s in the scratch the caller reserved there, statuses computed on the device
+// (device_forms.cuh).  The H(m) hints are those launch_verify_tail takes: same_msg / h_msg from a host form (it sees the messages),
+// mg from a device form (messages grouped on the device).
+// triples: keys decoded on the device, verdicts into d_results; d_status (nullable) receives the HBLS_VB_* codes
+static void verify_triples_body(size_t k, const uint8_t* d_pk, const uint8_t* d_sig, const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results,
+                                uint8_t* d_status, cudaStream_t s, Scratch* sc, Arena& ar, bool same_msg, const MsgGroups* mg) {
+    VerifyBufs v = carve_verify(ar, k);
+    fork_point(k, sc, s);
+    STAGE_EV(0, sc, s);
+    // keys stay Jacobian (z = 1): the same tail as a mask aggregate, so independent triples also go through the batched groups
+    LAUNCH(k_g1_decode_jac, heavy_blocks(k), TPB, s, k, d_pk, v.apk, v.ok_pk, 1);
+    launch_verify_tail(k, v, sc, d_sig, d_msgs, (uint32_t)msg_len, v.ok_pk, d_results, s, same_msg, nullptr, mg);
+    if (!d_status) return;
+    uint8_t* dflags = ar.take<uint8_t>(k);
+    LAUNCH(k_pack_flags, blocks_for(k, 256), 256, s, k, v.ok_sig, v.ok_hm, (const uint8_t*)v.ok_pk, dflags);
+    LAUNCH(k_status_triples, blocks_for(k, 256), 256, s, k, (const uint8_t*)dflags, (const uint8_t*)d_results, d_status);
+}
+// header ranges against one committee: HBLS_HDR_* codes into d_status
+static void verify_headers_body(const hbls_committee* c, size_t n, const uint8_t* d_sigs, const uint8_t* d_bitmaps, size_t blen,
+                                const uint8_t* d_payloads, size_t payload_len, size_t quorum, uint8_t* d_status, cudaStream_t s, Scratch* sc,
+                                Arena& ar, bool same_msg, const uint8_t* h_msg, const MsgGroups* mg) {
+    uint8_t* dres = ar.take<uint8_t>(n); uint8_t* dflags = ar.take<uint8_t>(n);
+    VerifyBufs v;
+    agg_verify_device_locked(c, n, d_bitmaps, blen, d_sigs, d_payloads, payload_len, dres, s, sc, ar, same_msg, &v, h_msg, mg);
+    LAUNCH(k_pack_flags, blocks_for(n, 256), 256, s, n, v.ok_sig, v.ok_hm, (const uint8_t*)nullptr, dflags);
+    LAUNCH(k_status_headers, blocks_for(n, 256), 256, s, n, c->n, d_bitmaps, blen, quorum, (const uint8_t*)dflags, (const uint8_t*)dres, d_status);
+}
+// items of a multi-committee batch (their bitmaps back to back in d_bitmaps): verdicts into d_results.  The descriptors (table,
+// bitmap, slots per item) come from the host array of handles.  They are written into the stream's own pinned buffer and uploaded
+// with an asynchronous copy; an event recorded after that copy guards the buffer, so a later call on the same stream waits (on the
+// host) only if the earlier upload has not run yet.  A pageable copy would synchronise the stream.
+static int verify_items_body(size_t k, const hbls_committee* const* committees, const uint8_t* d_bitmaps, const uint8_t* d_sigs,
+                             const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, Arena& ar, bool same_msg,
+                             const MsgGroups* mg) {
+    if (sc->items_pending) { CK(cudaEventSynchronize(sc->items_copied)); sc->items_pending = false; }
+    if (!sc->items_copied) CK(cudaEventCreateWithFlags(&sc->items_copied, cudaEventDisableTiming));
+    if (k > sc->h_items_cap) {
+        if (sc->h_items) CK(cudaFreeHost(sc->h_items));
+        sc->h_items = nullptr; sc->h_items_cap = 0;
+        CK(cudaMallocHost(&sc->h_items, k * sizeof(mask_item)));
+        sc->h_items_cap = k;
+    }
+    VerifyBufs v = carve_verify(ar, k);
+    mask_item* ditems = ar.take<mask_item>(k);
+    size_t off = 0;
+    for (size_t j = 0; j < k; j++) {
+        sc->h_items[j].table = committees[j]->table; sc->h_items[j].bitmap = d_bitmaps + off; sc->h_items[j].n = committees[j]->n;
+        off += (committees[j]->n + 7) >> 3;
+    }
+    CK(cudaMemcpyAsync(ditems, sc->h_items, k * sizeof(mask_item), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(sc->items_copied, s)); sc->items_pending = true;
+    fork_point(k, sc, s);
+    STAGE_EV(0, sc, s);
+    LAUNCH(k_mask_aggregate_items, blocks_for(k * 32, 128), 128, s, k, (const mask_item*)ditems, v.apk);
+    launch_verify_tail(k, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, same_msg, nullptr, mg);
+    return 0;
+}
+
+// ------------------------------------------------------------------ host forms: the inputs staged on g.stream, one synchronise
+// rounds against one committee: verdicts into out (hbls_aggregate_verify_batch); with `status`, the HBLS_HDR_* codes under quorum
+// (hbls_verify_headers).  One message for all rounds: it keys the H(m) cache.
 static int agg_verify_host_locked(const hbls_committee* c, size_t B, const uint8_t* bitmaps, size_t blen, const uint8_t* sigs96,
-                                  const uint8_t* msgs, size_t msg_len, uint8_t* results, uint8_t* flags_out) {
-    size_t in_bytes = B * (blen + 96 + msg_len);
-    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(B) + in_bytes + 2 * B + 4096, &sc)) return e;
+                                  const uint8_t* msgs, size_t msg_len, uint8_t* out, bool status = false, size_t quorum = 0) {
+    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(B) + B * (blen + 96 + msg_len + 3) + 4096, &sc)) return e;
     ensure_stage_events(sc);
     Arena ar{sc->base, 0, sc->cap};
     uint8_t* dbm = ar.take<uint8_t>(B * blen + 1); uint8_t* dsig = ar.take<uint8_t>(B * 96); uint8_t* dmsg = ar.take<uint8_t>(B * msg_len + 1);
-    uint8_t* dres = ar.take<uint8_t>(B); uint8_t* dflags = ar.take<uint8_t>(B);
+    uint8_t* dout = ar.take<uint8_t>(B);
     if (blen) CK(cudaMemcpyAsync(dbm, bitmaps, B * blen, cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(dsig, sigs96, B * 96, cudaMemcpyHostToDevice, g.stream));
     if (msg_len) CK(cudaMemcpyAsync(dmsg, msgs, B * msg_len, cudaMemcpyHostToDevice, g.stream));
-    VerifyBufs v;
     const bool same = all_messages_equal(msgs, B, msg_len);
-    agg_verify_device_locked(c, B, dbm, blen, dsig, dmsg, msg_len, dres, g.stream, sc, ar, same, &v, (same || B == 1) ? msgs : nullptr);
-    CK(cudaMemcpyAsync(results, dres, B, cudaMemcpyDeviceToHost, g.stream));
-    if (flags_out) {
-        LAUNCH(k_pack_flags, blocks_for(B, 256), 256, g.stream, B, v.ok_sig, v.ok_hm, (const uint8_t*)nullptr, dflags);
-        CK(cudaMemcpyAsync(flags_out, dflags, B, cudaMemcpyDeviceToHost, g.stream));
-    }
+    const uint8_t* h_msg = (same || B == 1) ? msgs : nullptr;
+    if (status) verify_headers_body(c, B, dsig, dbm, blen, dmsg, msg_len, quorum, dout, g.stream, sc, ar, same, h_msg, nullptr);
+    else agg_verify_device_locked(c, B, dbm, blen, dsig, dmsg, msg_len, dout, g.stream, sc, ar, same, nullptr, h_msg);
+    CK(cudaMemcpyAsync(out, dout, B, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
     return 0;
 }
@@ -1236,7 +1293,7 @@ int hbls_aggregate_verify_batch(const hbls_committee* c, size_t B, const uint8_t
     if (!c || blen != ((c->n + 7) >> 3)) return HBLS_ERR_ARG;
     if (B == 0) return 0;
     std::lock_guard<std::mutex> lk(g.mu);
-    return agg_verify_host_locked(c, B, bitmaps, blen, sigs96, msgs, msg_len, results, nullptr);
+    return agg_verify_host_locked(c, B, bitmaps, blen, sigs96, msgs, msg_len, results);
 }
 int hbls_aggregate_verify(const hbls_committee* c, const uint8_t* bitmap, size_t blen, const uint8_t sig96[96], const void* msg, size_t msg_len) {
     uint8_t res = 0;
@@ -1244,25 +1301,14 @@ int hbls_aggregate_verify(const hbls_committee* c, const uint8_t* bitmap, size_t
     if (rc) return rc;
     return res ? 1 : 0;
 }
-static int verify_headers_locked(const hbls_committee* c, size_t n, const uint8_t* sigs96, const uint8_t* bitmaps, size_t blen,
-                        const uint8_t* payloads, size_t payload_len, size_t quorum, uint8_t* status) {
-    std::vector<uint8_t> res(n), flags(n);
-    if (int e = agg_verify_host_locked(c, n, bitmaps, blen, sigs96, payloads, payload_len, res.data(), flags.data())) return e;
-    for (size_t i = 0; i < n; i++) {
-        // engine.go:630-640: DecodeSigBitmap (signature deserialise) -> IsQuorumAchievedByMask -> VerifyHash
-        if (!(flags[i] & 1)) status[i] = HBLS_HDR_BAD_ENCODING;
-        else if (quorum && (size_t)popcount_slots(bitmaps + i * blen, c->n) < quorum) status[i] = HBLS_HDR_NO_QUORUM;
-        else status[i] = res[i] ? HBLS_HDR_OK : HBLS_HDR_BAD_SIG;
-    }
-    return 0;
-}
+// engine.go:630-640: DecodeSigBitmap (signature deserialise) -> IsQuorumAchievedByMask -> VerifyHash
 int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96, const uint8_t* bitmaps, size_t blen,
                         const uint8_t* payloads, size_t payload_len, size_t quorum, uint8_t* status) {
     if (int e = ensure_init()) return e;
     if (!c || blen != ((c->n + 7) >> 3) || !status) return HBLS_ERR_ARG;        // DecodeSigBitmap: mask.SetMask length error (sig.go:43)
     if (n == 0) return 0;
     std::lock_guard<std::mutex> lk(g.mu);
-    return verify_headers_locked(c, n, sigs96, bitmaps, blen, payloads, payload_len, quorum, status);
+    return agg_verify_host_locked(c, n, bitmaps, blen, sigs96, payloads, payload_len, status, true, quorum);
 }
 
 static int aggregate_verify_items_locked(size_t k, const hbls_committee* const* committees, const uint8_t* bitmaps, const uint8_t* sigs96,
@@ -1272,21 +1318,14 @@ static int aggregate_verify_items_locked(size_t k, const hbls_committee* const* 
     Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(k) + bm_bytes + k * (96 + msg_len + 1 + sizeof(mask_item)) + 4096, &sc)) return e;
     ensure_stage_events(sc);
     Arena ar{sc->base, 0, sc->cap};
-    VerifyBufs v = carve_verify(ar, k);
     uint8_t* dbm = ar.take<uint8_t>(bm_bytes + 1); uint8_t* dsig = ar.take<uint8_t>(k * 96); uint8_t* dmsg = ar.take<uint8_t>(k * msg_len + 1);
-    uint8_t* dres = ar.take<uint8_t>(k); mask_item* ditems = ar.take<mask_item>(k);
-    std::vector<mask_item> items(k); size_t off = 0;
-    for (size_t j = 0; j < k; j++) { items[j].table = committees[j]->table; items[j].bitmap = dbm + off; items[j].n = committees[j]->n; off += (committees[j]->n + 7) >> 3; }
+    uint8_t* dres = ar.take<uint8_t>(k);
     if (bm_bytes) CK(cudaMemcpyAsync(dbm, bitmaps, bm_bytes, cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(dsig, sigs96, k * 96, cudaMemcpyHostToDevice, g.stream));
     if (msg_len) CK(cudaMemcpyAsync(dmsg, msgs, k * msg_len, cudaMemcpyHostToDevice, g.stream));
-    CK(cudaMemcpyAsync(ditems, items.data(), k * sizeof(mask_item), cudaMemcpyHostToDevice, g.stream));
-    fork_point(k, sc, g.stream);
-    STAGE_EV(0, sc, g.stream);
-    LAUNCH(k_mask_aggregate_items, blocks_for(k * 32, 128), 128, g.stream, k, ditems, v.apk);
-    launch_verify_tail(k, v, sc, dsig, dmsg, (uint32_t)msg_len, nullptr, dres, g.stream, all_messages_equal(msgs, k, msg_len));
+    if (int e = verify_items_body(k, committees, dbm, dsig, dmsg, msg_len, dres, g.stream, sc, ar, all_messages_equal(msgs, k, msg_len), nullptr)) return e;
     CK(cudaMemcpyAsync(results, dres, k, cudaMemcpyDeviceToHost, g.stream));
-    CK(cudaStreamSynchronize(g.stream));          // items[] (pageable source of an async copy) stays alive until here
+    CK(cudaStreamSynchronize(g.stream));
     return 0;
 }
 int hbls_aggregate_verify_items(size_t k, const hbls_committee* const* committees, const uint8_t* bitmaps, const uint8_t* sigs96,
@@ -1299,27 +1338,19 @@ int hbls_aggregate_verify_items(size_t k, const hbls_committee* const* committee
     return aggregate_verify_items_locked(k, committees, bitmaps, sigs96, msgs, msg_len, results);
 }
 
-// shared body of hbls_verify_batch / hbls_verify_batch_status; flags_out (nullable): k_pack_flags bytes per item
-static int verify_batch_locked(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* results, uint8_t* flags_out) {
-    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(k) + k * (48 + 96 + msg_len + 2) + 4096, &sc)) return e;
+// hbls_verify_batch: verdicts into out; with `status`, hbls_verify_batch_status: the caller learns WHY an item failed, in the order
+// the reference meets the errors (k_status_triples)
+static int verify_batch_locked(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* out, bool status) {
+    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(k) + k * (48 + 96 + msg_len + 3) + 4096, &sc)) return e;
     ensure_stage_events(sc);
     Arena ar{sc->base, 0, sc->cap};
-    VerifyBufs v = carve_verify(ar, k);
     uint8_t* dpk = ar.take<uint8_t>(k * 48); uint8_t* dsig = ar.take<uint8_t>(k * 96); uint8_t* dmsg = ar.take<uint8_t>(k * msg_len + 1);
-    uint8_t* dres = ar.take<uint8_t>(k); uint8_t* dflags = ar.take<uint8_t>(k);
+    uint8_t* dres = ar.take<uint8_t>(k); uint8_t* dst = status ? ar.take<uint8_t>(k) : nullptr;
     CK(cudaMemcpyAsync(dpk, pk48, k * 48, cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(dsig, sig96, k * 96, cudaMemcpyHostToDevice, g.stream));
     if (msg_len) CK(cudaMemcpyAsync(dmsg, msgs, k * msg_len, cudaMemcpyHostToDevice, g.stream));
-    fork_point(k, sc, g.stream);
-    STAGE_EV(0, sc, g.stream);
-    // keys stay Jacobian (z = 1): the same tail as a mask aggregate, so independent triples also go through the batched groups
-    LAUNCH(k_g1_decode_jac, heavy_blocks(k), TPB, g.stream, k, dpk, v.apk, v.ok_pk, 1);
-    launch_verify_tail(k, v, sc, dsig, dmsg, (uint32_t)msg_len, v.ok_pk, dres, g.stream, all_messages_equal(msgs, k, msg_len));
-    CK(cudaMemcpyAsync(results, dres, k, cudaMemcpyDeviceToHost, g.stream));
-    if (flags_out) {
-        LAUNCH(k_pack_flags, blocks_for(k, 256), 256, g.stream, k, v.ok_sig, v.ok_hm, (const uint8_t*)v.ok_pk, dflags);
-        CK(cudaMemcpyAsync(flags_out, dflags, k, cudaMemcpyDeviceToHost, g.stream));
-    }
+    verify_triples_body(k, dpk, dsig, dmsg, msg_len, dres, dst, g.stream, sc, ar, all_messages_equal(msgs, k, msg_len), nullptr);
+    CK(cudaMemcpyAsync(out, status ? dst : dres, k, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
     return 0;
 }
@@ -1327,45 +1358,26 @@ int hbls_verify_batch(size_t k, const uint8_t* pk48, const uint8_t* sig96, const
     if (int e = ensure_init()) return e;
     if (k == 0) return 0;
     std::lock_guard<std::mutex> lk(g.mu);
-    return verify_batch_locked(k, pk48, sig96, msgs, msg_len, results, nullptr);
-}
-// same check, but the caller learns WHY an item failed, in the order the reference meets the errors: the sender key is decoded
-// first (BytesToBLSPublicKey, consensus/view_change_msg.go:159), then the signature (Sign.Deserialize, :168-179), then VerifyHash
-static int verify_batch_status_locked(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* status) {
-    std::vector<uint8_t> flags(k);
-    if (int e = verify_batch_locked(k, pk48, sig96, msgs, msg_len, status, flags.data())) return e;
-    for (size_t j = 0; j < k; j++) {
-        if (!(flags[j] & 4)) status[j] = HBLS_VB_BAD_KEY_ENCODING;
-        else if (!(flags[j] & 1)) status[j] = HBLS_VB_BAD_SIG_ENCODING;
-        else status[j] = status[j] == 1 ? HBLS_VB_OK : HBLS_VB_BAD_SIG;
-    }
-    return 0;
+    return verify_batch_locked(k, pk48, sig96, msgs, msg_len, results, false);
 }
 int hbls_verify_batch_status(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* status) {
     if (int e = ensure_init()) return e;
     if (k == 0) return 0;
     if (!status) return HBLS_ERR_ARG;
     std::lock_guard<std::mutex> lk(g.mu);
-    return verify_batch_status_locked(k, pk48, sig96, msgs, msg_len, status);
+    return verify_batch_locked(k, pk48, sig96, msgs, msg_len, status, true);
 }
 
-// ------------------------------------------------------------------ device forms of the three batch verifiers above: inputs and
-// outputs in HBM (any byte alignment), everything enqueued on the caller's stream with no host synchronisation, statuses computed
-// on the device (device_forms.cuh), H(m) once per distinct message (grouped on the device; the H(m) cache is neither read nor
-// filled: the host never sees the messages).  Same kernels and batching regimes as the host forms otherwise.
+// ------------------------------------------------------------------ device forms: inputs and outputs in HBM (any byte alignment),
+// everything enqueued on the caller's stream with no host synchronisation, H(m) once per distinct message (grouped on the device;
+// the H(m) cache is neither read nor filled: the host never sees the messages)
 static int verify_batch_status_device_locked(size_t k, const uint8_t* d_pk, const uint8_t* d_sig, const uint8_t* d_msgs, size_t msg_len,
                                              uint8_t* d_status, cudaStream_t s) {
     Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(k) + group_bytes(k) + 2 * k + 4096, &sc)) return e;
     ensure_stage_events(sc);
     Arena ar{sc->base, 0, sc->cap};
-    VerifyBufs v = carve_verify(ar, k); const MsgGroups mg = carve_groups(ar, k);
-    uint8_t* dres = ar.take<uint8_t>(k); uint8_t* dflags = ar.take<uint8_t>(k);
-    fork_point(k, sc, s);
-    STAGE_EV(0, sc, s);
-    LAUNCH(k_g1_decode_jac, heavy_blocks(k), TPB, s, k, d_pk, v.apk, v.ok_pk, 1);
-    launch_verify_tail(k, v, sc, d_sig, d_msgs, (uint32_t)msg_len, v.ok_pk, dres, s, false, nullptr, &mg);
-    LAUNCH(k_pack_flags, blocks_for(k, 256), 256, s, k, v.ok_sig, v.ok_hm, (const uint8_t*)v.ok_pk, dflags);
-    LAUNCH(k_status_triples, blocks_for(k, 256), 256, s, k, (const uint8_t*)dflags, (const uint8_t*)dres, d_status);
+    const MsgGroups mg = carve_groups(ar, k); uint8_t* dres = ar.take<uint8_t>(k);
+    verify_triples_body(k, d_pk, d_sig, d_msgs, msg_len, dres, d_status, s, sc, ar, false, &mg);
     CK(cudaGetLastError());
     return 0;
 }
@@ -1383,11 +1395,7 @@ static int verify_headers_device_locked(const hbls_committee* c, size_t n, const
     ensure_stage_events(sc);
     Arena ar{sc->base, 0, sc->cap};
     const MsgGroups mg = carve_groups(ar, n);
-    uint8_t* dres = ar.take<uint8_t>(n); uint8_t* dflags = ar.take<uint8_t>(n);
-    VerifyBufs v;
-    agg_verify_device_locked(c, n, d_bitmaps, blen, d_sigs, d_payloads, payload_len, dres, s, sc, ar, false, &v, nullptr, &mg);
-    LAUNCH(k_pack_flags, blocks_for(n, 256), 256, s, n, v.ok_sig, v.ok_hm, (const uint8_t*)nullptr, dflags);
-    LAUNCH(k_status_headers, blocks_for(n, 256), 256, s, n, c->n, d_bitmaps, blen, quorum, (const uint8_t*)dflags, (const uint8_t*)dres, d_status);
+    verify_headers_body(c, n, d_sigs, d_bitmaps, blen, d_payloads, payload_len, quorum, d_status, s, sc, ar, false, nullptr, &mg);
     CK(cudaGetLastError());
     return 0;
 }
@@ -1400,35 +1408,13 @@ int hbls_verify_headers_device(const hbls_committee* c, size_t n, const void* d_
     return verify_headers_device_locked(c, n, (const uint8_t*)d_sigs96, (const uint8_t*)d_bitmaps, blen, (const uint8_t*)d_payloads, payload_len, quorum,
                                         (uint8_t*)d_status, stream ? (cudaStream_t)stream : g.stream);
 }
-// The descriptors (table, bitmap, slots per item) come from the host array of handles.  They are written into the stream's own pinned
-// buffer and uploaded with an asynchronous copy; an event recorded after that copy guards the buffer, so a later call on the same
-// stream waits (on the host) only if the earlier upload has not run yet.  A pageable copy would synchronise the stream.
 static int aggregate_verify_items_device_locked(size_t k, const hbls_committee* const* committees, const uint8_t* d_bitmaps, const uint8_t* d_sigs,
                                                 const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s) {
     Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(k) + group_bytes(k) + k * sizeof(mask_item) + 4096, &sc)) return e;
     ensure_stage_events(sc);
-    if (sc->items_pending) { CK(cudaEventSynchronize(sc->items_copied)); sc->items_pending = false; }
-    if (!sc->items_copied) CK(cudaEventCreateWithFlags(&sc->items_copied, cudaEventDisableTiming));
-    if (k > sc->h_items_cap) {
-        if (sc->h_items) CK(cudaFreeHost(sc->h_items));
-        sc->h_items = nullptr; sc->h_items_cap = 0;
-        CK(cudaMallocHost(&sc->h_items, k * sizeof(mask_item)));
-        sc->h_items_cap = k;
-    }
     Arena ar{sc->base, 0, sc->cap};
-    VerifyBufs v = carve_verify(ar, k); const MsgGroups mg = carve_groups(ar, k);
-    mask_item* ditems = ar.take<mask_item>(k);
-    size_t off = 0;
-    for (size_t j = 0; j < k; j++) {
-        sc->h_items[j].table = committees[j]->table; sc->h_items[j].bitmap = d_bitmaps + off; sc->h_items[j].n = committees[j]->n;
-        off += (committees[j]->n + 7) >> 3;
-    }
-    CK(cudaMemcpyAsync(ditems, sc->h_items, k * sizeof(mask_item), cudaMemcpyHostToDevice, s));
-    CK(cudaEventRecord(sc->items_copied, s)); sc->items_pending = true;
-    fork_point(k, sc, s);
-    STAGE_EV(0, sc, s);
-    LAUNCH(k_mask_aggregate_items, blocks_for(k * 32, 128), 128, s, k, (const mask_item*)ditems, v.apk);
-    launch_verify_tail(k, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, false, nullptr, &mg);
+    const MsgGroups mg = carve_groups(ar, k);
+    if (int e = verify_items_body(k, committees, d_bitmaps, d_sigs, d_msgs, msg_len, d_results, s, sc, ar, false, &mg)) return e;
     CK(cudaGetLastError());
     return 0;
 }

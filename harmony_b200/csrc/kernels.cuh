@@ -348,26 +348,29 @@ __global__ void k_hash_to_g2(size_t n, const uint8_t* msgs, uint32_t msg_len, g2
 #ifndef HB_SW_MINBLOCKS
 #define HB_SW_MINBLOCKS 8         // x 64 threads = 512 resident threads per SM (<= 128 registers)
 #endif
-__global__ void __launch_bounds__(64, HB_SW_MINBLOCKS) k_hash_sw(size_t n, const uint8_t* msgs, uint32_t msg_len, g2a* pts, uint8_t* ok) {
-  for (size_t i0 = HB_TID; i0 < n; i0 += (size_t)HB_BATCH_K * HB_STRIDE) {
+// thread form, one thread's HB_BATCH_K items i0 + j * HB_STRIDE: the SW maps of the items below n share one inversion; items in
+// [n, k) get the identity with ok = 0
+HB_DEV void hash_sw_items(size_t i0, size_t n, size_t k, const uint8_t* msgs, uint32_t msg_len, g2a* pts, uint8_t* ok) {
     fp2 z[HB_BATCH_K], t[HB_BATCH_K], u[HB_BATCH_K], ct[HB_BATCH_K]; bool skip[HB_BATCH_K];
-    for (int k = 0; k < HB_BATCH_K; k++) {
-        const size_t i = i0 + (size_t)k * HB_STRIDE;
-        skip[k] = true;
+    for (int j = 0; j < HB_BATCH_K; j++) {
+        const size_t i = i0 + (size_t)j * HB_STRIDE;
+        skip[j] = true;
         if (i >= n) continue;
-        fp_zero(t[k].b); hash_to_fp(t[k].a, msgs + (size_t)msg_len * i, msg_len);
-        skip[k] = !sw_map_g2_pre(u[k], ct[k], z[k], t[k]);
+        fp_zero(t[j].b); hash_to_fp(t[j].a, msgs + (size_t)msg_len * i, msg_len);
+        skip[j] = !sw_map_g2_pre(u[j], ct[j], z[j], t[j]);
     }
     f_batch_inv<fp2, HB_BATCH_K>(z, skip);
-    for (int k = 0; k < HB_BATCH_K; k++) {
-        const size_t i = i0 + (size_t)k * HB_STRIDE;
-        if (i >= n) continue;
+    for (int j = 0; j < HB_BATCH_K; j++) {
+        const size_t i = i0 + (size_t)j * HB_STRIDE;
+        if (i >= k) continue;
         g2 a; g2a o; fp2_zero(o.x); fp2_zero(o.y);
-        const bool good = !skip[k] && sw_map_g2_post(a, t[k], u[k], ct[k], z[k]);
+        const bool good = !skip[j] && sw_map_g2_post(a, t[j], u[j], ct[j], z[j]);
         if (good) { o.x = a.x; o.y = a.y; }
         pts[i] = o; ok[i] = good ? 1 : 0;
     }
-  }
+}
+__global__ void __launch_bounds__(64, HB_SW_MINBLOCKS) k_hash_sw(size_t n, const uint8_t* msgs, uint32_t msg_len, g2a* pts, uint8_t* ok) {
+    for (size_t i0 = HB_TID; i0 < n; i0 += (size_t)HB_BATCH_K * HB_STRIDE) hash_sw_items(i0, n, n, msgs, msg_len, pts, ok);
 }
 // cofactor clearing alone, Jacobian result (no per-thread arrays of pending items: the frame is the group law's own temporaries), and
 // the shared-inversion affine conversion as its own small kernel.  hbls.cu runs the cofactor clearing as k_hash_cofactor_pair; this
@@ -437,52 +440,58 @@ __global__ void k_g2_decode_pair(size_t n, const uint8_t* in, g2a* out, uint8_t*
         out[i] = a; ok[i] = good ? 1 : 0;
     }
 }
+// The per-item bodies of the lane-pair and warp forms of hash-to-G2, shared by the message kernels below and the key kernels of
+// device_forms.cuh.  They are macros, not functions: a function boundary, even a forceinline one, changes the stack layout ptxas is
+// given, and with it the registers and spills of these latency-path kernels.
+// The lane-pair tail: cofactor clearing of the mapped point a on the split carrier, binary-GCD inversion, affine result into res
+// (left as it is -- zero -- for the identity).
+#define HB_HASH_TAIL_PAIR(res, a) {                                                                                                   \
+        jac<fp2h> A, H; fp2h_pack(A.x, a.x); fp2h_pack(A.y, a.y); fp2h_pack(A.z, a.z);                                              \
+        g2_clear_cofactor(H, A);                                                                                                      \
+        if (!pt_is_inf(H)) {                                                                                                          \
+            fp2h zi, zi2, hx, hy; fp2_inv_gcd(zi, H.z); fp2_sqr(zi2, zi);                                                            \
+            fp2_mul(hx, H.x, zi2); fp2_mul(zi2, zi2, zi); fp2_mul(hy, H.y, zi2);                                                     \
+            fp2h_unpack(res.x, hx); fp2h_unpack(res.y, hy);                                                                          \
+        }                                                                                                                             \
+    }
+// lane-pair form: message i (msg_len bytes at stride msg_len) on the calling lane pair (both lanes compute the same point: the map
+// is Fp-heavy), the even lane writes
+#define HB_HASH_ITEM_PAIR(i, msgs, msg_len, out, ok) {                                                                                \
+    fp2 t; hash_to_fp(t.a, msgs + (size_t)msg_len * i, msg_len); fp_zero(t.b);                                                       \
+    g2 a; bool good = sw_map_g2<true>(a, t);                                                                                          \
+    g2a res; fp2_zero(res.x); fp2_zero(res.y);                                                                                        \
+    if (good) HB_HASH_TAIL_PAIR(res, a)                                                                                               \
+    if ((threadIdx.x & 1) == 0) { out[i] = res; ok[i] = good ? 1 : 0; }                                                              \
+}
 __global__ void k_hash_to_g2_pair(size_t n, const uint8_t* msgs, uint32_t msg_len, g2a* out, uint8_t* ok) {
     const size_t i = HB_TID >> 1; if (i >= n) return;
-    fp2 t; hash_to_fp(t.a, msgs + (size_t)msg_len * i, msg_len); fp_zero(t.b);
-    g2 a; bool good = sw_map_g2<true>(a, t);                              // Fp-heavy: both lanes compute the same point
-    g2a res; fp2_zero(res.x); fp2_zero(res.y);
-    if (good) {
-        jac<fp2h> A, H; fp2h_pack(A.x, a.x); fp2h_pack(A.y, a.y); fp2h_pack(A.z, a.z);
-        g2_clear_cofactor(H, A);
-        if (!pt_is_inf(H)) {
-            fp2h zi, zi2, hx, hy; fp2_inv_gcd(zi, H.z); fp2_sqr(zi2, zi);
-            fp2_mul(hx, H.x, zi2); fp2_mul(zi2, zi2, zi); fp2_mul(hy, H.y, zi2);
-            fp2h_unpack(res.x, hx); fp2h_unpack(res.y, hy);
-        }
-    }
-    if ((threadIdx.x & 1) == 0) { out[i] = res; ok[i] = good ? 1 : 0; }
+    HB_HASH_ITEM_PAIR(i, msgs, msg_len, out, ok)
 }
 // ---- latency form of hash-to-G2 (vm.cuh): ONE WARP per message.  The Shallue-van de Woestijne map (Fp chains: one inversion, two
-// Legendre symbols, the Fp2 square root) runs on every lane alike; the cofactor clearing -- two 63-doubling chains of G2, about half
-// of a lane pair's hash time -- runs as VM step programs with the 3 independent products of a doubling level
-// side by side.  Falls back to the complete lane-pair code when the generic formulas degenerate.
+// Legendre symbols, the Fp2 square root) runs on every lane alike (warp-uniform: every lane maps the same message); the cofactor
+// clearing -- two 63-doubling chains of G2, about half of a lane pair's hash time -- runs as VM step programs with the 3 independent
+// products of a doubling level side by side.  Falls back to the complete lane-pair code when the generic formulas degenerate
+// (force_fallback: test hook, hbls_set_param "hash_fallback").  Message i on the calling warp, whose VM slots hold the constants
+// (vm_load_consts); lane 0 writes.
+#define HB_HASH_ITEM_WARP(i, msgs, msg_len, out, ok, slots, lane, force_fallback) {                                                  \
+        fp2 t; hash_to_fp(t.a, msgs + (size_t)msg_len * i, msg_len); fp_zero(t.b);                                                   \
+        g2 a; const bool good = sw_map_g2<true>(a, t);                                                                                \
+        g2a res; fp2_zero(res.x); fp2_zero(res.y);                                                                                    \
+        if (good) {                                                                                                                   \
+            if (lane == 0) { vm_set_fp2(slots, VM_R_Q2X, a.x); vm_set_fp2(slots, VM_R_Q2Y, a.y); }                                   \
+            __syncwarp();                                                                                                             \
+            if (vm_hash_cofactor(slots) && !force_fallback) {                                                                         \
+                if (lane == 0) { vm_ld(res.x.a.l, slots, VM_R_HX, 0); vm_ld(res.x.b.l, slots, VM_R_HX, 1); vm_ld(res.y.a.l, slots, VM_R_HY, 0); vm_ld(res.y.b.l, slots, VM_R_HY, 1); } \
+            } else if (lane < 2) HB_HASH_TAIL_PAIR(res, a)                                                                            \
+        }                                                                                                                             \
+        if (lane == 0) { out[i] = res; ok[i] = good ? 1 : 0; }                                                                       \
+        __syncwarp();                                                                                                                 \
+    }
 __global__ void __launch_bounds__(32) k_hash_to_g2_coop(size_t n, const uint8_t* msgs, uint32_t msg_len, g2a* out, uint8_t* ok, int force_fallback) {
     __shared__ uint32_t slots[VM_SMEM_WORDS];
     const int lane = threadIdx.x & 31;
     vm_load_consts(slots);
-    for (size_t i = blockIdx.x; i < n; i += gridDim.x) {
-        fp2 t; hash_to_fp(t.a, msgs + (size_t)msg_len * i, msg_len); fp_zero(t.b);
-        g2 a; const bool good = sw_map_g2<true>(a, t);                       // warp-uniform: every lane maps the same message
-        g2a res; fp2_zero(res.x); fp2_zero(res.y);
-        if (good) {
-            if (lane == 0) { vm_set_fp2(slots, VM_R_Q2X, a.x); vm_set_fp2(slots, VM_R_Q2Y, a.y); }
-            __syncwarp();
-            if (vm_hash_cofactor(slots) && !force_fallback) {             // force_fallback: test hook (hbls_set_param "hash_fallback")
-                if (lane == 0) { vm_ld(res.x.a.l, slots, VM_R_HX, 0); vm_ld(res.x.b.l, slots, VM_R_HX, 1); vm_ld(res.y.a.l, slots, VM_R_HY, 0); vm_ld(res.y.b.l, slots, VM_R_HY, 1); }
-            } else if (lane < 2) {
-                jac<fp2h> A, H; fp2h_pack(A.x, a.x); fp2h_pack(A.y, a.y); fp2h_pack(A.z, a.z);
-                g2_clear_cofactor(H, A);
-                if (!pt_is_inf(H)) {
-                    fp2h zi, zi2, hx, hy; fp2_inv_gcd(zi, H.z); fp2_sqr(zi2, zi);
-                    fp2_mul(hx, H.x, zi2); fp2_mul(zi2, zi2, zi); fp2_mul(hy, H.y, zi2);
-                    fp2h_unpack(res.x, hx); fp2h_unpack(res.y, hy);
-                }
-            }
-        }
-        if (lane == 0) { out[i] = res; ok[i] = good ? 1 : 0; }
-        __syncwarp();
-    }
+    for (size_t i = blockIdx.x; i < n; i += gridDim.x) HB_HASH_ITEM_WARP(i, msgs, msg_len, out, ok, slots, lane, force_fallback)
 }
 
 // same-message batches (the leader's prepare / commit vote collection, consensus/leader.go:127-290: every vote signs

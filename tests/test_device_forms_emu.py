@@ -1,7 +1,9 @@
 """CPU-only: the message-grouping and status kernels of harmony_b200/csrc/device_forms.cuh run on the host
 (tests/emu/emu_device_forms.cpp).  Grouping: items whose messages agree in the 48 zero-padded bytes the map reads are one message,
-represented by their lowest index, numbered in item order, whatever order the "threads" run in.  Statuses: the order of checks of
-hbls.cu verify_batch_status_locked / verify_headers_locked, restated here, on every combination of the k_pack_flags bits."""
+represented by their lowest index, numbered in item order, whatever order the "threads" run in.  Statuses: the status kernels are
+the only library code that assigns HBLS_VB_* / HBLS_HDR_*, for the host and the device forms alike; the order of checks (key, then signature
+encoding, then VerifyHash; encoding, then quorum, then VerifyHash) is restated independently here and checked on every combination
+of the k_pack_flags bits."""
 import ctypes, itertools, os, random, subprocess
 import pytest
 

@@ -1,6 +1,6 @@
 """tools/device_entries_time.py -- host forms of the batch verifiers against their device forms, alternating in one process.
 
-Host form: host bytes in, statuses on the host (hbls_verify_batch_status / hbls_aggregate_verify_items / hbls_verify_headers).
+Host form: host bytes in, statuses copied back to the host (hbls_verify_batch_status / hbls_aggregate_verify_items / hbls_verify_headers).
 Device form: the same inputs already in HBM as uint8 CUDA tensors, statuses in HBM (the *_device entry points), timed up to a
 torch.cuda.synchronize() after the call plus the copy of the statuses back for the comparison.  Host clock around each call; median and range of --reps calls after a warm-up call of
 each.  The H(m) cache is off (hm_cache 0) for both, so the host forms do not reuse the previous repetition's H(m).
