@@ -269,6 +269,33 @@ template <class F> HB_NOINLINE void pt_mul_2d_aff_jsf(jac<F>& r, const aff<F>& p
     r = acc;
 }
 
+// ---- r = sum_t [k_t] P_t over N (affine point, 32-bit scalar) pairs with ONE shared accumulator (Straus): every k_t in non-adjacent
+// form (<= 33 signed digits, 11.4 of them non-zero on average), so the N ladders share their 33 doublings and a non-zero digit costs
+// one mixed addition of +-P_t.  load(t, q) yields P_t and is called once per non-zero digit: no table, no Jacobian temporaries.  The
+// digits depend on the scalars alone, so callers whose warps share them stay divergence-free.  Exceptional sums (an identity P_t,
+// acc == +-P_t) take pt_add_mixed's branches.
+// NAF by bit operations: np - nm == k with np & nm == 0 and no two adjacent non-zero digits (bit i of np / nm: digit i is +1 / -1)
+HB_DEV void naf_masks(uint32_t k, uint64_t& np, uint64_t& nm) {
+    const uint64_t x = k, xh = x >> 1, x3 = x + xh, c = xh ^ x3;
+    np = x3 & c; nm = xh & c;
+}
+template <class E, int N, class Load> HB_NOINLINE void pt_mul_joint_naf(jac<E>& r, const uint32_t* k, Load load) {
+    jac<E> acc; pt_set_inf(acc);
+    for (int i = 32; i >= 0; i--) {
+        HB_USYNC();
+        pt_dbl(acc, acc);
+#pragma unroll 1
+        for (int t = 0; t < N; t++) {
+            uint64_t np, nm; naf_masks(k[t], np, nm);
+            if ((((np | nm) >> i) & 1) == 0) continue;
+            aff<E> q; load(t, q);
+            if ((nm >> i) & 1) f_neg(q.y, q.y);
+            pt_add_mixed(acc, acc, q);
+        }
+    }
+    r = acc;
+}
+
 HB_DEV void g1_generator(g1& r) { fp_set(r.x, K_G1_X); fp_set(r.y, K_G1_Y); fp_one(r.z); }
 
 // ------------------------------------------------------------------ endomorphisms and subgroup membership

@@ -50,6 +50,8 @@ struct Ctx {
     long long rlc_min = 12288, rlc_g = 0, tpsm = 384, tpsm_split = 512, tpsm_light = 1024, coop_max = 4096, overlap = 1, coop_wpsm = 14, hash_coop_max = 528, mask_sort = 1, hash_split = 2, tpsm_sw = 512, hash_fallback = 0, rlc_two_phase = 2, tpsm_lines = 512, tpsm_accum = 512, tpsm_cof = 512, tpsm_dec = 512, tpsm_sub = 512, tpsm_scale = 384, tpsm_scale_g2 = 512, tpsm_scale_g1 = 384, scale_split = 1, decode_split = 1, exact_two_phase = 1;
     int* rlc_form = nullptr;                                // device: 1 = the last call that could use blocks had many failed groups (k_rlc_form)
     long long rlc_block = 0;                                // blocks of HB_RLC_M groups (rlc_blocks): 0 automatic, 1 forced on, 2 forced off
+    long long scale_joint = 1;                              // signature scaling: 0 a ladder per round + group sums, 1 one joint ladder per group
+                                                            // once the groups fill the chip, 2 always the joint ladder
     // coefficient stream: ChaCha20 keyed from /dev/urandom, block counter = call number
     uint32_t chacha_key[8] = {}; uint64_t rlc_calls = 0;
     // last batch
@@ -436,14 +438,22 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
         // group form's / block form's kernels, the scaling kernels take the matching coefficients
         const unsigned* blk_gate = blocks ? v.counts + 3 : nullptr;
         if (blocks) LAUNCH(k_rlc_form, 1, 32, s, ng, g.rlc_block == 1 ? 1 : 0, (const int*)g.rlc_form, v.counts + 2);
+        bool joint = false;
         if (g.scale_split && HB_BATCH_INV) {
             LAUNCH(k_rlc_scale_g1, capped_blocks(nr, g.tpsm_scale_g1, TPB), TPB, s, nr, ng, v.apk, co, v.pk_scaled, S, cb, blk_gate);
             const unsigned t = lockstep_cta(g.tpsm_scale_g2);
-            LAUNCH(k_rlc_scale_g2_pair, capped_blocks(2 * nr, t, t), t, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+            // the joint ladder runs a lane pair per GROUP: G times fewer items than the per-round ladder, so it needs a full chip of groups
+            joint = g.scale_joint >= 2 || (g.scale_joint == 1 && full);
+            if (joint) {          // one ladder per group into the Jacobian Sg (the first ng entries of S), then the shared-inversion affine form
+                if (G == 8) LAUNCH(k_rlc_group_scale_g2_pair<8>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+                else LAUNCH(k_rlc_group_scale_g2_pair<4>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+                LAUNCH(k_g2_normalize_batch, heavy_blocks(ng), TPB, s, ng, (const g2*)v.S, v.Sg);
+            } else
+                LAUNCH(k_rlc_scale_g2_pair, capped_blocks(2 * nr, t, t), t, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
         } else
         LAUNCH(k_rlc_scale, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, (const uint64_t*)nullptr, v.pk_scaled, v.S, v.bad, S, cb, blk_gate);
-        if (G == 8) LAUNCH(k_rlc_group_sum<8>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
-        else LAUNCH(k_rlc_group_sum<4>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
+        if (!joint && G == 8) LAUNCH(k_rlc_group_sum<8>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
+        else if (!joint) LAUNCH(k_rlc_group_sum<4>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
         STAGE_EV(5, sc, s);
         if (two_phase) {
             // running points in their own kernel (lines to HBM, read once), accumulator + final exponentiation in the second
@@ -956,7 +966,7 @@ int hbls_init_device(int device) {
         CK(cudaEventCreateWithFlags(&g.hm[i].filled, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&g.hm[i].read_done, cudaEventDisableTiming));
     }
     g.hm_cache = envll("HBLS_HM_CACHE", 1); g.mask_sort = envll("HBLS_MASK_SORT", 1); g.hash_coop_max = envll("HBLS_HASH_COOP_MAX", 4ll * g.sm_count);     // one warp per message while every scheduler gets one
-    g.rlc_two_phase = envll("HBLS_RLC_2P", 2); g.tpsm_lines = envll("HBLS_TPSM_LINES", 512); g.tpsm_accum = envll("HBLS_TPSM_ACCUM", 512); g.tpsm_cof = envll("HBLS_TPSM_COF", 512); g.tpsm_dec = envll("HBLS_TPSM_DEC", 512); g.tpsm_sub = envll("HBLS_TPSM_SUB", 512); g.tpsm_scale = envll("HBLS_TPSM_SCALE", 384); g.tpsm_scale_g1 = envll("HBLS_TPSM_SCALE_G1", 384); g.tpsm_scale_g2 = envll("HBLS_TPSM_SCALE_G2", 512); g.scale_split = envll("HBLS_SCALE_SPLIT", 1); g.decode_split = envll("HBLS_DECODE_SPLIT", 1); g.exact_two_phase = envll("HBLS_EXACT_2P", 1);
+    g.rlc_two_phase = envll("HBLS_RLC_2P", 2); g.tpsm_lines = envll("HBLS_TPSM_LINES", 512); g.tpsm_accum = envll("HBLS_TPSM_ACCUM", 512); g.tpsm_cof = envll("HBLS_TPSM_COF", 512); g.tpsm_dec = envll("HBLS_TPSM_DEC", 512); g.tpsm_sub = envll("HBLS_TPSM_SUB", 512); g.tpsm_scale = envll("HBLS_TPSM_SCALE", 384); g.tpsm_scale_g1 = envll("HBLS_TPSM_SCALE_G1", 384); g.tpsm_scale_g2 = envll("HBLS_TPSM_SCALE_G2", 512); g.scale_split = envll("HBLS_SCALE_SPLIT", 1); g.scale_joint = envll("HBLS_SCALE_JOINT", 1); g.decode_split = envll("HBLS_DECODE_SPLIT", 1); g.exact_two_phase = envll("HBLS_EXACT_2P", 1);
     g.rlc_block = envll("HBLS_RLC_BLOCK", 0);
     g.hash_split = envll("HBLS_HASH_SPLIT", 2); g.tpsm_sw = envll("HBLS_TPSM_SW", 512);
     CK(cudaFuncSetAttribute(k_hash_sw, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
@@ -984,7 +994,7 @@ const ParamDef PARAMS[] = {
     {"overlap", &Ctx::overlap}, {"coop_wpsm", &Ctx::coop_wpsm}, {"hm_cache", &Ctx::hm_cache}, {"hash_coop_max", &Ctx::hash_coop_max}, {"mask_sort", &Ctx::mask_sort}, {"hash_split", &Ctx::hash_split},
     {"hash_fallback", &Ctx::hash_fallback}, {"rlc_two_phase", &Ctx::rlc_two_phase}, {"tpsm_cof", &Ctx::tpsm_cof}, {"tpsm_dec", &Ctx::tpsm_dec}, {"tpsm_sub", &Ctx::tpsm_sub}, {"tpsm_scale", &Ctx::tpsm_scale}, {"tpsm_scale_g1", &Ctx::tpsm_scale_g1}, {"tpsm_scale_g2", &Ctx::tpsm_scale_g2},
     {"scale_split", &Ctx::scale_split}, {"decode_split", &Ctx::decode_split}, {"exact_two_phase", &Ctx::exact_two_phase}, {"tpsm_lines", &Ctx::tpsm_lines}, {"tpsm_accum", &Ctx::tpsm_accum}, {"tpsm_sw", &Ctx::tpsm_sw},
-    {"rlc_block", &Ctx::rlc_block}, {"selftest_flip", &Ctx::selftest_flip}};
+    {"rlc_block", &Ctx::rlc_block}, {"scale_joint", &Ctx::scale_joint}, {"selftest_flip", &Ctx::selftest_flip}};
 static long long* param_slot(const char* name) {
     if (!name) return nullptr;
     for (const ParamDef& p : PARAMS) if (!strcmp(name, p.name)) return &(g.*p.slot);
@@ -995,7 +1005,7 @@ int hbls_set_param(const char* name, long long value) {
     long long* p = param_slot(name);
     if (!p || value < 0) return HBLS_ERR_ARG;
     if (p == &g.rlc_g && value != 0 && value != 4 && value != 8) return HBLS_ERR_ARG;
-    if (p == &g.rlc_block && value > 2) return HBLS_ERR_ARG;
+    if ((p == &g.rlc_block || p == &g.scale_joint) && value > 2) return HBLS_ERR_ARG;
     *p = value; return 0;
 }
 long long hbls_get_param(const char* name) { std::lock_guard<std::mutex> lk(g.mu); long long* p = param_slot(name); return p ? *p : -1; }

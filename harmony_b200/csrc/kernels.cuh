@@ -998,6 +998,39 @@ template <int G> __global__ void k_rlc_group_sum(size_t ngroups, const g2* S, g2
     g2a a; pt_to_aff(a, acc); Sg[g] = a;
   }
 }
+// k_rlc_scale_g2_pair + k_rlc_group_sum<G> as ONE joint ladder per group (hbls.cu "scale_joint"): the pairing stage reads the rounds'
+// scaled signatures only through their group sum Sg = sum_k s_k sigma_k, so a lane pair runs pt_mul_joint_naf over the group's 2G
+// half-scalars (a_k on sigma_k, b_k on psi^2 sigma_k, split as in rlc_scale_g2) and its rounds share 33 doublings instead of running
+// a ladder each.  The unit coefficient is (a, b) = (1, 0): one addition of sigma_k.  Writes the Jacobian Sg (k_g2_normalize_batch
+// turns it affine) and the bad flag of each of the G rounds, by k_rlc_scale_g2_pair's rule.  A warp's 16 pairs hold 16 consecutive
+// groups, which share every coefficient (per position, or per (position, member) with the member stride a multiple of 32), so the
+// digits stay warp-uniform.
+template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_group_scale_g2_pair(size_t ng, const g1* apk, const g2a* sig,
+        const g2a* hm, const uint8_t* ok_sig, const uint8_t* ok_hm, const uint8_t* ok_pk, rlc_coeffs co, g2* Sg, uint8_t* bad,
+        size_t blk_stride = 0, rlc_block_coeffs cb = {}, const unsigned* blk_gate = nullptr) {
+  if (blk_gate && *blk_gate == 0) blk_stride = 0;
+  const int role = threadIdx.x & 1;
+  pair_sweep(ng, [&](size_t g) {
+    uint32_t k[2 * G];
+    for (int t = 0; t < G; t++) {
+        const size_t j = (size_t)t * ng + g;
+        const uint64_t c = rlc_coeff(co, j, ng, blk_stride, cb);
+        k[2 * t] = (uint32_t)c | 1u; k[2 * t + 1] = (uint32_t)(c >> 32);
+        const fp* s4 = reinterpret_cast<const fp*>(&sig[j]);
+        const fp* h4 = reinterpret_cast<const fp*>(&hm[j]);
+        aff<fp2h> sg, h; sg.x.c = s4[role]; sg.y.c = s4[2 + role]; h.x.c = h4[role]; h.y.c = h4[2 + role];
+        const bool b = !ok_sig[j] || !ok_hm[j] || (ok_pk && !ok_pk[j]) || fp_is_zero(apk[j].z) || aff_is_inf(sg) || aff_is_inf(h);
+        if (role == 0) bad[j] = b ? 1 : 0;
+    }
+    jac<fp2h> acc;
+    pt_mul_joint_naf<fp2h, 2 * G>(acc, k, [&](int t, aff<fp2h>& q) {
+        const fp* s4 = reinterpret_cast<const fp*>(&sig[(size_t)(t >> 1) * ng + g]);
+        q.x.c = s4[role]; q.y.c = s4[2 + role];
+        if (t & 1) { fp2_mul_fp(q.x, q.x, fp_k(K_PSI2_CX)); fp2_neg(q.y, q.y); }      // psi^2(x, y) = (N(cx) x, -y)
+    });
+    fp* o = reinterpret_cast<fp*>(&Sg[g]); o[role] = acc.x.c; o[2 + role] = acc.y.c; o[4 + role] = acc.z.c;
+  });
+}
 #ifndef HB_SMEM_F
 #define HB_SMEM_F 0       // 1: keep each lane's Fp12 accumulator in dynamic shared memory (experiment, not faster)
 #endif

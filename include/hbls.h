@@ -144,7 +144,9 @@ int hbls_last_batch_info(hbls_batch_info* out);
  * checks of at most this many rounds use the warp-per-round latency kernel, 0 = never), "tpsm" (resident threads per SM of the
  * thread-per-item kernels), "tpsm_split" (lane-pair kernels), "tpsm_light", "coop_wpsm" (resident warps per SM of the warp-per-round kernels), "hm_cache" (0: H(m) cache off), "hash_coop_max" (hash-to-G2 of at most this many messages runs one warp per message), "mask_sort" (1: large batches aggregate keys in the order of the rounds' addition counts), "hash_split" (large batches hash in 0: one kernel, 1: map + cofactor clearing, 2: map + cofactor clearing + affine conversion), "rlc_two_phase" (batched pairing as 0: one kernel, 1: two kernels when the batch fills the chip, 2: always two kernels), "hash_fallback" (test hook: 1 forces the warp-per-message hash through its complete-formula fall-back), "tpsm_sw" (resident threads per SM of the map kernel), "overlap" (1: small batches decode signatures and
  * hash messages on two auxiliary streams beside the key aggregation), "rlc_block" (blocks of 16 groups sharing one final
- * exponentiation: 0 automatic, 1 forced on wherever they can run, 2 off; default from HBLS_RLC_BLOCK).  Defaults come from HBLS_RLC_MIN, HBLS_RLC_G, HBLS_COOP_MAX,
+ * exponentiation: 0 automatic, 1 forced on wherever they can run, 2 off; default from HBLS_RLC_BLOCK), "scale_joint" (signature scaling
+ * as 0: a ladder per round + group sums, 1: one joint ladder per group when the groups fill the chip, 2: always the joint ladder;
+ * default from HBLS_SCALE_JOINT).  Defaults come from HBLS_RLC_MIN, HBLS_RLC_G, HBLS_COOP_MAX,
  * HBLS_TPSM, HBLS_TPSM_SPLIT, HBLS_TPSM_LIGHT at blsInit.  0 ok, HBLS_ERR_ARG for an unknown name / bad value. */
 int hbls_set_param(const char* name, long long value);
 long long hbls_get_param(const char* name);
@@ -306,7 +308,7 @@ int hbls_selftest_split(uint32_t iters);
 /* per-kernel device timing of the aggregate-verify pipeline (CUDA events on the launching stream).
  * enable(1) makes every following hbls_aggregate_verify_batch[_device] call record events between its kernels;
  * get() waits for the last recorded pipeline and returns the number of stages written to ms_out, in launch order:
- * 0 mask aggregation, 1 (-apk to affine; exact mode only), 2 k_g2_decode, 3 k_hash_to_g2, 4 k_rlc_scale + k_rlc_group_sum, 5 pairing
+ * 0 mask aggregation, 1 (-apk to affine; exact mode only), 2 k_g2_decode, 3 k_hash_to_g2, 4 k_rlc_scale + k_rlc_group_sum (or the joint ladder + k_g2_normalize_batch), 5 pairing
  * (batched groups + exact pass over failed groups; in exact mode stage 4 is empty) */
 void hbls_stage_timing_enable(int on);
 int hbls_stage_timing_get(float* ms_out, int max_stages);
