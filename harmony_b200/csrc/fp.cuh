@@ -51,9 +51,6 @@
 #define HB_FP2FN __device__ __forceinline__
 #endif
 
-#ifndef HB_CARRY2
-#define HB_CARRY2 1      // 1: ripple every lane-chain carry two limbs up (measured faster than the provably sufficient single limb: ptxas schedules it better)
-#endif
 
 namespace hb {
 
@@ -120,12 +117,10 @@ HB_DEV void lane_mad(uint32_t* acc, const uint32_t* a, uint32_t b) {
         madc_lo_cc(acc[j], a[j], b, acc[j]);
         madc_hi_cc(acc[j + 1], a[j], b, acc[j + 1]);
     }
-#if HB_CARRY2
+    // the carry ripples two limbs up: the windows accumulate several rows, and a single limb measured wrong results on the
+    // device (tests/test_arith_primitives.py)
     addc_cc(acc[12], acc[12], 0);
     addc(acc[13], acc[13], 0);
-#else
-    addc(acc[12], acc[12], 0);       // a partial sum never reaches limb 13 of its window (it is bounded by a * 2^(32 rows))
-#endif
 }
 // same with the modulus (limbs become immediates), PAR = 0 even limbs, 1 odd limbs
 template <int PAR> HB_DEV void lane_mad_p(uint32_t* acc, uint32_t m) {
@@ -136,12 +131,8 @@ template <int PAR> HB_DEV void lane_mad_p(uint32_t* acc, uint32_t m) {
         madc_lo_cc(acc[j], p_limb(PAR + j), m, acc[j]);
         madc_hi_cc(acc[j + 1], p_limb(PAR + j), m, acc[j + 1]);
     }
-#if HB_CARRY2
     addc_cc(acc[12], acc[12], 0);
     addc(acc[13], acc[13], 0);
-#else
-    addc(acc[12], acc[12], 0);
-#endif
 }
 
 // r = a*b/R mod p, inputs and output canonical in [0, p)

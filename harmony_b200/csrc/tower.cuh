@@ -425,9 +425,12 @@ HB_DEV void fp2_const(fp2h& r, const uint32_t k[2][12]) { fp_set(r.c, k[fp2h_rol
 template <class E> HB_DEV const E& fp2_k(const uint32_t k[2][12]);
 template <> HB_DEV const fp2& fp2_k<fp2>(const uint32_t k[2][12]) { return fp2_k(k); }
 template <> HB_DEV const fp2h& fp2_k<fp2h>(const uint32_t k[2][12]) { return *reinterpret_cast<const fp2h*>(k[fp2h_role()]); }
+// both lanes always reach the exchange: with `mine && shfl(..)` a lane whose own half differs skipped it, and its partner then
+// waited on a shuffle the pair did not execute together (a difference confined to one half, e.g. in pt_eq of the subgroup test)
 HB_DEV bool fp2_eq(const fp2h& x, const fp2h& y) {
     const int mine = fp_eq(x.c, y.c) ? 1 : 0;
-    return mine && __shfl_xor_sync(HB_PAIR_MASK, mine, 1) != 0;
+    const int other = __shfl_xor_sync(HB_PAIR_MASK, mine, 1);
+    return mine && other;
 }
 HB_DEV void fp2_cmov(fp2h& r, const fp2h& x, bool c) { fp_cmov(r.c, x.c, c); }
 // whole value <-> the pair's halves (both lanes end up holding the full Fp2 element / each lane keeps its own half)
