@@ -23,6 +23,9 @@ struct Request {
 
 struct Stats { uint64_t turns = 0, requests = 0, max_turn = 0; };
 
+// every kind counts against its own cap
+struct OwnCap { int operator()(int kind) const { return kind; } };
+
 class Combiner {
 public:
     static constexpr int kMaxKinds = 8;
@@ -31,8 +34,9 @@ public:
     //   outer:    locked by the leader before it drains the queue (requests that arrive while another holder has it join the turn)
     //   cap(k):   most requests of kind k in one turn (read with `outer` held; 0 counts as 1); the rest wait for the next turn
     //   exec(rq, n): runs one turn on the leader's thread with `outer` held; must complete every one of the n requests
-    template <class Outer, class Cap, class Exec>
-    void submit(Request& r, Outer& outer, Cap&& cap, Exec&& exec) {
+    //   pool(k):  the kind whose cap a request of kind k counts against (kinds that share one device stage share one cap)
+    template <class Outer, class Cap, class Exec, class Pool = OwnCap>
+    void submit(Request& r, Outer& outer, Cap&& cap, Exec&& exec, Pool&& pool = Pool{}) {
         std::unique_lock<std::mutex> lk(mu_);
         queue_.push_back(&r);
         for (;;) {
@@ -48,7 +52,8 @@ public:
                 lk.lock();
                 std::deque<Request*> rest;
                 for (Request* q : queue_) {
-                    if (taken[q->kind] < caps[q->kind]) { taken[q->kind]++; turn.push_back(q); }
+                    const int p = pool(q->kind);
+                    if (taken[p] < caps[p]) { taken[p]++; turn.push_back(q); }
                     else rest.push_back(q);
                 }
                 queue_.swap(rest);

@@ -2,6 +2,7 @@
 // Host side = plumbing only (buffers, streams, launches); every group/field operation runs on the GPU.
 // No CPU fallback exists: without a usable CUDA device blsInit fails and every entry point returns HBLS_ERR_CUDA.
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
@@ -19,6 +20,19 @@
 #include "device_forms.cuh"
 
 using namespace hb;
+
+struct hbls_committee {
+    size_t n = 0;
+    g1a* table = nullptr;       // device, affine, Montgomery
+    g1* total = nullptr;        // device, sum of all rows (lets dense bitmaps be aggregated from their complement)
+    ~hbls_committee() { if (table) cudaFree(table); if (total) cudaFree(total); }
+};
+struct hbls_mask {
+    const hbls_committee* c = nullptr;
+    std::vector<uint8_t> bitmap;        // Mask.Bitmap (host)
+    g1* d_acc = nullptr;                // Mask.AggregatePublic (device, Jacobian)
+    ~hbls_mask() { if (d_acc) cudaFree(d_acc); }
+};
 
 namespace {
 
@@ -597,17 +611,24 @@ bool scalar_lt_r(const uint64_t k[4]) {
 // time.  Concurrent calls from different threads are combined into turns (coalesce.hpp); a turn stages the inputs of all its requests
 // with one copy, runs each kernel once over the requests that need it and copies the results back once.  A lone call is a turn of
 // one and launches the kernels a call has always launched.
-enum { RQ_VERIFY, RQ_SIGN, RQ_PUBKEY, RQ_SINGLE };
+// The single checks against a committee (hbls_aggregate_verify: AGG) and a resident mask (hbls_mask_verify: MASK) join the same
+// turns: with VERIFY they are the turn's verify requests and share its warp-per-round cap.
+enum { RQ_VERIFY, RQ_SIGN, RQ_PUBKEY, RQ_SINGLE, RQ_AGG, RQ_MASK };
 constexpr size_t PART1_CAP = 1024;       // sign / GetPublicKey / single-element requests per turn (verify: coop_max, the warp-per-round limit)
 struct Part1Req : hbls_coalesce::Request {
-    const void* a = nullptr; const void* b = nullptr;   // VERIFY: signature, public key; SIGN / PUBKEY: secret key; SINGLE: operands
+    const void* a = nullptr; const void* b = nullptr;   // VERIFY: signature, public key; AGG / MASK: the serialized signature (96 bytes);
+                                                        // SIGN / PUBKEY: secret key; SINGLE: operands
     size_t an = 0, bn = 0;                              // SINGLE: operand bytes
-    const void* msg = nullptr; size_t len = 0;          // VERIFY / SIGN: the hash (first 48 bytes); SINGLE: the message length
+    const void* msg = nullptr; size_t len = 0;          // VERIFY / AGG / MASK / SIGN: the hash (first 48 bytes); SINGLE: the message length
     void* out = nullptr; size_t on = 0;                 // SIGN / PUBKEY: the result struct; SINGLE: the result bytes
+    const hbls_committee* com = nullptr;                // AGG: the committee, and the bitmap of blen = (n + 7) / 8 bytes
+    const uint8_t* bitmap = nullptr; size_t blen = 0;
+    const hbls_mask* mask = nullptr;                    // MASK: the mask whose resident aggregate key is checked
     int op = 0;                                         // SINGLE: OP_*
     int err = 0;                                        // HBLS_ERR_CUDA when the turn's device work failed (nothing written)
-    int rc = 0;                                         // VERIFY: 1 / 0; SIGN: 0 / -1; SINGLE: the op's return code
+    int rc = 0;                                         // VERIFY / AGG / MASK: 1 / 0; SIGN: 0 / -1; SINGLE: the op's return code
 };
+static bool is_verify(int kind) { return kind == RQ_VERIFY || kind == RQ_AGG || kind == RQ_MASK; }
 static_assert(sizeof(g1) == sizeof(blsPublicKey) && sizeof(g2) == sizeof(blsSignature), "herumi struct layout");
 // byte layout of one staging copy: 256-byte aligned sections
 struct Layout {
@@ -615,13 +636,23 @@ struct Layout {
     size_t put(size_t bytes) { const size_t off = (size + 255) & ~(size_t)255; size = off + (bytes ? bytes : 1); return off; }
 };
 
-// One turn: the requests rq[0..n) under g.mu.  d_apk / sig96 (hbls_mask_verify: one verify request): the key is already on the
-// device and the signature is serialized (decoded and subgroup-checked here).  Fills in each request's results and returns 0, or
-// HBLS_ERR_CUDA with no result written.
+// One turn: the requests rq[0..n) under g.mu.  d_apk / sig96 (a lone hbls_mask_verify: one verify request): the key is already on
+// the device and the signature is serialized (decoded and subgroup-checked here).  Otherwise the verify requests run in the order
+// AGG, MASK, VERIFY through one pipeline: their keys land in one array of Jacobian keys inside the staging buffer (AGG: summed from
+// the committee tables by k_mask_aggregate_items, MASK: the resident aggregate copied device to device, VERIFY: staged), the AGG /
+// MASK signatures are decoded with the subgroup test and the VERIFY structs made affine, then one pairing launch checks them all.
+// Fills in each request's results and returns 0, or HBLS_ERR_CUDA with no result written.
 int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const uint8_t* sig96 = nullptr) {
     cudaStream_t s = g.stream;
     std::vector<Part1Req*> ver, sgn, pub, one;
-    for (size_t i = 0; i < n; i++) (rq[i]->kind == RQ_VERIFY ? ver : rq[i]->kind == RQ_SIGN ? sgn : rq[i]->kind == RQ_PUBKEY ? pub : one).push_back(rq[i]);
+    for (size_t i = 0; i < n; i++) (is_verify(rq[i]->kind) ? ver : rq[i]->kind == RQ_SIGN ? sgn : rq[i]->kind == RQ_PUBKEY ? pub : one).push_back(rq[i]);
+    auto vrank = [](int kind) { return kind == RQ_AGG ? 0 : kind == RQ_MASK ? 1 : 2; };
+    std::stable_sort(ver.begin(), ver.end(), [&](const Part1Req* x, const Part1Req* y) { return vrank(x->kind) < vrank(y->kind); });
+    size_t na = 0, nser = 0;                            // AGG requests; AGG + MASK requests (serialized signatures)
+    for (const Part1Req* r : ver) { na += r->kind == RQ_AGG; nser += r->kind != RQ_VERIFY; }
+    if (d_apk) na = nser = 0;
+    size_t bm_bytes = 0;
+    for (size_t i = 0; i < na; i++) bm_bytes += ver[i]->blen;
     // signing keys in base |z| first (ladder over psi), hand-filled keys >= Z^4 after them (plain ladder)
     std::vector<uint64_t> dig; size_t ngls = 0;
     {
@@ -655,7 +686,10 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     for (size_t i = 0; i < nh; i++) { idx[i] = pos[idx[i]]; gather |= idx[i] != i; }
     // staging (host -> device, one copy) and results (device -> host, one copy)
     Layout in, out;
-    const size_t i_apk = d_apk ? 0 : in.put(nv * sizeof(g1)), i_sig = in.put(sig96 ? 96 : nv * sizeof(g2)), i_keys = in.put(nmiss * 48);
+    const size_t i_apk = d_apk ? 0 : in.put(nv * sizeof(g1)), i_sig = in.put(sig96 ? 96 : (nv - nser) * sizeof(g2)), i_keys = in.put(nmiss * 48);
+    // AGG / MASK: the serialized signatures, the decode flags of every verify request, the mask_item descriptors and their bitmaps
+    const size_t i_ser = nser ? in.put(nser * 96) : 0, i_sok = nser ? in.put(nv) : 0;
+    const size_t i_items = na ? in.put(na * sizeof(mask_item)) : 0, i_bm = na ? in.put(bm_bytes) : 0;
     const size_t i_idx = gather ? in.put(nh * 4) : 0, i_dig = in.put(dig.size() * 8), i_sk = in.put((ns - ngls) * 32), i_pub = in.put(np * 32);
     std::vector<size_t> i_a(n1), i_b(n1), o_out(n1);
     for (size_t j = 0; j < n1; j++) { i_a[j] = in.put(one[j]->an); i_b[j] = in.put(one[j]->bn); o_out[j] = out.put(one[j]->on); }
@@ -669,9 +703,20 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     g2a* hm = ar.take<g2a>(nh); uint8_t* ok_hm = ar.take<uint8_t>(nh);
     g2a* th = gather ? ar.take<g2a>(nk) : hm; uint8_t* tok = gather ? ar.take<uint8_t>(nk) : ok_hm;      // the H(m) table
     std::vector<uint8_t> hin(in.size), hout(out.size);
-    for (size_t i = 0; i < nv && !d_apk; i++) memcpy(&hin[i_apk + i * sizeof(g1)], ver[i]->b, sizeof(g1));
+    for (size_t i = nser; i < nv && !d_apk; i++) memcpy(&hin[i_apk + i * sizeof(g1)], ver[i]->b, sizeof(g1));
     if (sig96) memcpy(&hin[i_sig], sig96, 96);
-    else for (size_t i = 0; i < nv; i++) memcpy(&hin[i_sig + i * sizeof(g2)], ver[i]->a, sizeof(g2));
+    else for (size_t i = nser; i < nv; i++) memcpy(&hin[i_sig + (i - nser) * sizeof(g2)], ver[i]->a, sizeof(g2));
+    if (nser) {
+        for (size_t i = 0; i < nser; i++) memcpy(&hin[i_ser + 96 * i], ver[i]->a, 96);
+        memset(&hin[i_sok], 1, nv);                      // VERIFY structs count as decoded; the decode writes the first nser flags
+        for (size_t i = 0, off = 0; i < na; i++) {
+            const Part1Req& r = *ver[i];
+            const mask_item it{r.com->table, din + i_bm + off, (uint64_t)r.com->n};
+            memcpy(&hin[i_items + i * sizeof(mask_item)], &it, sizeof it);
+            if (r.blen) memcpy(&hin[i_bm + off], r.bitmap, r.blen);
+            off += r.blen;
+        }
+    }
     for (size_t d = 0; d < nk; d++) if (!cached[d]) memcpy(&hin[i_keys + 48 * pos[d]], keys[d].data(), 48);
     if (gather) memcpy(&hin[i_idx], idx.data(), nh * 4);
     if (!dig.empty()) memcpy(&hin[i_dig], dig.data(), dig.size() * 8);
@@ -690,9 +735,15 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     if (np) LAUNCH(k_g1_mul_gen, blocks_for(np, 32), 32, s, np, (const uint8_t*)(din + i_pub), reinterpret_cast<g1*>(dout + o_pub));
     const uint8_t* vok_sig = nullptr;
     if (nv) {
-        LAUNCH(k_g1_normalize_lat, blocks_for(nv, 32), 32, s, nv, d_apk ? d_apk : reinterpret_cast<const g1*>(din + i_apk), pkneg, 1);
+        g1* apk = reinterpret_cast<g1*>(din + i_apk);
+        if (na) LAUNCH(k_mask_aggregate_items, blocks_for(na * 32, 128), 128, s, na, (const mask_item*)(din + i_items), apk);
+        for (size_t i = na; i < nser; i++) CK(cudaMemcpyAsync(apk + i, ver[i]->mask->d_acc, sizeof(g1), cudaMemcpyDeviceToDevice, s));
+        LAUNCH(k_g1_normalize_lat, blocks_for(nv, 32), 32, s, nv, d_apk ? d_apk : (const g1*)apk, pkneg, 1);
         if (sig96) { LAUNCH(k_g2_decode_pair, 1, 32, s, (size_t)1, (const uint8_t*)(din + i_sig), vsig, ok_sig, 1); vok_sig = ok_sig; }
-        else LAUNCH(k_g2_normalize, blocks_for(nv, 32), 32, s, nv, reinterpret_cast<const g2*>(din + i_sig), vsig);
+        else {
+            if (nser) { LAUNCH(k_g2_decode_pair, blocks_for(2 * nser, 32), 32, s, nser, (const uint8_t*)(din + i_ser), vsig, din + i_sok, 1); vok_sig = din + i_sok; }
+            if (nv > nser) LAUNCH(k_g2_normalize, blocks_for(nv - nser, 32), 32, s, nv - nser, reinterpret_cast<const g2*>(din + i_sig), vsig + nser);
+        }
     }
     // H(m): cached entries (this node signed, verified or prefetched the message before), then one launch over the misses
     for (size_t d = 0; d < nk; d++) if (cached[d]) hm_fetch(keys[d].data(), th + pos[d], tok + pos[d], s);
@@ -716,6 +767,12 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(hout.data(), dout, out.size, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
+    if (na) {            // committee checks in the turn: an exact-mode batch of na rounds, a warp per round (hbls_last_batch_info)
+        g.info = hbls_batch_info{}; g.info.mode = 0; g.info.rounds = na; g.info.cta_threads = 32;
+        sc->h_counts[0] = sc->h_counts[1] = 0;
+        CK(cudaEventRecord(sc->done, s));
+        g.info_sc = sc; g.info_valid = true;
+    }
     for (size_t i = 0; i < nv; i++) ver[i]->rc = hout[o_res + i] ? 1 : 0;
     for (size_t i = 0; i < ns; i++) { memcpy(sgn[i]->out, &hout[o_sig + i * sizeof(g2)], sizeof(g2)); sgn[i]->rc = hout[o_sok + i] ? 0 : -1; }
     for (size_t i = 0; i < np; i++) memcpy(pub[i]->out, &hout[o_pub + i * sizeof(g1)], sizeof(g1));
@@ -727,16 +784,24 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     return 0;
 }
 
-// runs r in a turn of the combiner (from any thread; the caller must not hold g.mu)
+int agg_verify_one_locked(Part1Req& r);       // a lone AGG request: the path of hbls_aggregate_verify_batch with one round
+
+// runs r in a turn of the combiner (from any thread; the caller must not hold g.mu).  A turn of one AGG or MASK request runs the
+// launches its call made before it could be combined: the three-stream latency path of one round, or part1_locked on the mask's key.
 void part1_submit(Part1Req& r) {
     g.part1.submit(r, g.mu,
         [](int kind) { return kind == RQ_VERIFY ? (size_t)(g.coop_max > 0 ? g.coop_max : 1) : PART1_CAP; },
         [](hbls_coalesce::Request** rq, size_t n) {
             std::vector<Part1Req*> turn(n);
             for (size_t i = 0; i < n; i++) turn[i] = static_cast<Part1Req*>(rq[i]);
-            const int e = part1_locked(turn.data(), n);
+            Part1Req& r0 = *turn[0];
+            int e;
+            if (n == 1 && r0.kind == RQ_AGG) e = agg_verify_one_locked(r0);
+            else if (n == 1 && r0.kind == RQ_MASK) e = part1_locked(turn.data(), 1, r0.mask->d_acc, static_cast<const uint8_t*>(r0.a));
+            else e = part1_locked(turn.data(), n);
             for (Part1Req* r : turn) r->err = e;
-        });
+        },
+        [](int kind) { return is_verify(kind) ? (int)RQ_VERIFY : kind; });
 }
 int single_op(int op, const void* a, size_t an, const void* b, size_t bn, void* out, size_t on, int* rc_out, uint32_t len = 0) {
     if (int e = ensure_init()) return e;
@@ -827,18 +892,6 @@ struct Sha512 {
 
 }  // namespace
 
-struct hbls_committee {
-    size_t n = 0;
-    g1a* table = nullptr;       // device, affine, Montgomery
-    g1* total = nullptr;        // device, sum of all rows (lets dense bitmaps be aggregated from their complement)
-    ~hbls_committee() { if (table) cudaFree(table); if (total) cudaFree(total); }
-};
-struct hbls_mask {
-    const hbls_committee* c = nullptr;
-    std::vector<uint8_t> bitmap;        // Mask.Bitmap (host)
-    g1* d_acc = nullptr;                // Mask.AggregatePublic (device, Jacobian)
-    ~hbls_mask() { if (d_acc) cudaFree(d_acc); }
-};
 struct hbls_ballot_box {
     const hbls_committee* c = nullptr;
     std::vector<uint8_t> collected;     // signers already counted
@@ -1305,11 +1358,13 @@ int hbls_aggregate_verify_batch(const hbls_committee* c, size_t B, const uint8_t
     std::lock_guard<std::mutex> lk(g.mu);
     return agg_verify_host_locked(c, B, bitmaps, blen, sigs96, msgs, msg_len, results);
 }
+// a single check: a request of the Part-1 combiner (concurrent callers share turns; a lone call is agg_verify_one_locked)
 int hbls_aggregate_verify(const hbls_committee* c, const uint8_t* bitmap, size_t blen, const uint8_t sig96[96], const void* msg, size_t msg_len) {
-    uint8_t res = 0;
-    int rc = hbls_aggregate_verify_batch(c, 1, bitmap, blen, sig96, (const uint8_t*)msg, msg_len, &res);
-    if (rc) return rc;
-    return res ? 1 : 0;
+    if (int e = ensure_init()) return e;
+    if (!c || blen != ((c->n + 7) >> 3) || !sig96) return HBLS_ERR_ARG;
+    Part1Req r; r.kind = RQ_AGG; r.com = c; r.bitmap = bitmap; r.blen = blen; r.a = sig96; r.msg = msg; r.len = msg_len;
+    part1_submit(r);
+    return r.err ? r.err : r.rc;
 }
 // engine.go:630-640: DecodeSigBitmap (signature deserialise) -> IsQuorumAchievedByMask -> VerifyHash
 int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96, const uint8_t* bitmaps, size_t blen,
@@ -1499,11 +1554,9 @@ int hbls_mask_get(const hbls_mask* m, uint8_t* bitmap_out, size_t blen, uint8_t 
 int hbls_mask_verify(const hbls_mask* m, const uint8_t sig96[96], const void* msg, size_t msg_len) {
     if (int e = ensure_init()) return e;
     if (!m || !sig96) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
-    Part1Req r; r.kind = RQ_VERIFY; r.msg = msg; r.len = msg_len;
-    Part1Req* rq = &r;
-    if (int e = part1_locked(&rq, 1, m->d_acc, sig96)) return e;
-    return r.rc;
+    Part1Req r; r.kind = RQ_MASK; r.mask = m; r.a = sig96; r.msg = msg; r.len = msg_len;
+    part1_submit(r);
+    return r.err ? r.err : r.rc;
 }
 int hbls_ballot_box_create(hbls_ballot_box** out, const hbls_committee* c) {
     if (int e = ensure_init()) return e;
@@ -1775,5 +1828,16 @@ double hbls_probe_mac32_per_s(int iters, double* sm_clock_hz) {
 }
 
 }  // extern "C"
+
+namespace {
+// a turn of one AGG request: exactly what hbls_aggregate_verify_batch does for one round (latency kernels on three streams, the H(m)
+// cache keyed by the message, the hbls_last_batch_info record)
+int agg_verify_one_locked(Part1Req& r) {
+    uint8_t res = 0;
+    if (int e = agg_verify_host_locked(r.com, 1, r.bitmap, r.blen, static_cast<const uint8_t*>(r.a), static_cast<const uint8_t*>(r.msg), r.len, &res)) return e;
+    r.rc = res ? 1 : 0;
+    return 0;
+}
+}  // namespace
 
 #include "selftest.cuh"

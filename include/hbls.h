@@ -12,10 +12,12 @@
  *
  * Conventions: plain pointers and sizes only; all memory caller-owned; no callbacks; int error codes.
  * Threading: every function may be called from any thread after blsInit.  Part-1 calls made concurrently (VerifyHash / Verify,
- * SignHash / Sign, GetPublicKey, Add / Sub, IsEqual, Serialize / Deserialize of keys and signatures, hbls_map_to_g2) are combined
- * into shared device launches: while one turn runs on the GPU, or a batch call holds it, the calls that arrive queue up and the next
- * caller in line runs them all as one turn (hbls_coalesce_stats counts the turns).  There is no timer or batching window: a call
- * that finds the library idle runs at once, alone, with the launches it has always made.  Device work is serialised by one library
+ * SignHash / Sign, GetPublicKey, Add / Sub, IsEqual, Serialize / Deserialize of keys and signatures, hbls_map_to_g2), and the single
+ * committee checks hbls_aggregate_verify and hbls_mask_verify, are combined into shared device launches: while one turn runs on the
+ * GPU, or a batch call holds it, the calls that arrive queue up and the next caller in line runs them all as one turn
+ * (hbls_coalesce_stats counts the turns).  VerifyHash and the two committee checks share one pairing launch and at most `coop_max`
+ * of them go into one turn.  There is no timer or batching window: a call that finds the library idle runs at once, alone, with
+ * the launches it has always made.  The batch entry points and the ballot box are not combined.  Device work is serialised by one library
  * mutex and (except the *_device entry points on a caller stream) one library stream.  Scratch memory is per stream, so
  * asynchronous device-pointer calls on DIFFERENT streams do not share intermediates; calls on one stream are stream-ordered.
  * Messages: only the first min(len, 48) bytes enter the map to G2 (mcl setArrayMask; SURVEY A.3); batch entry points take the
@@ -108,7 +110,9 @@ int hbls_aggregate_sigs(const uint8_t* sig96, size_t n, uint8_t out96[96]);
 
 /* FastAggregateVerify / VerifyAggregateSig of BASELINE.json == the reference composition
  * Deserialize(sig) ; SetMask(bitmap) ; aggSig.VerifyHash(mask.AggregatePublic, msg)
- * (internal/chain/engine.go:630-640, consensus/validator.go:219-236).  1 valid, 0 invalid, <0 error. */
+ * (internal/chain/engine.go:630-640, consensus/validator.go:219-236).  1 valid, 0 invalid, <0 error.  HBLS_ERR_ARG for a null
+ * committee or signature or blen != (n + 7) >> 3.  Concurrent calls share turns (threading, above); the handle must stay alive
+ * until the call returns. */
 int hbls_aggregate_verify(const hbls_committee* c, const uint8_t* bitmap, size_t blen,
                           const uint8_t sig96[96], const void* msg, size_t msg_len);
 
@@ -128,7 +132,10 @@ void hbls_set_batch_mode(int mode);
 int  hbls_get_batch_mode(void);
 /* what the most recent batch call (aggregate_verify_batch[_device], verify_batch, aggregate_verify_items, verify_headers,
  * ballot_box_submit_votes) did:
- * waits for that call's device work if it is still running.  0 ok, HBLS_ERR_ARG if no batch call was made yet. */
+ * waits for that call's device work if it is still running.  0 ok, HBLS_ERR_ARG if no batch call was made yet.
+ * hbls_aggregate_verify records a batch too: alone, the one-round batch it runs; in a turn shared with other calls, the turn's
+ * committee checks as one exact-mode batch (mode 0, rounds = the hbls_aggregate_verify calls of the turn, cta_threads 32: a warp
+ * per round).  hbls_mask_verify records none. */
 typedef struct {
     int32_t  mode;              /* 1: batched groups (+ exact pass over failed groups), 0: exact per round */
     int32_t  group_size;        /* G (4 or 8) in mode 1, else 0 */
@@ -226,7 +233,8 @@ int  hbls_mask_clear(hbls_mask* m);
 int  hbls_mask_count_enabled(const hbls_mask* m);
 /* bitmap_out (nullable, blen bytes) = Mask.Bitmap ; pk48_out (nullable) = AggregatePublic.Serialize() */
 int  hbls_mask_get(const hbls_mask* m, uint8_t* bitmap_out, size_t blen, uint8_t pk48_out[48]);
-/* aggSig.VerifyHash(mask.AggregatePublic, msg) with the resident aggregate (consensus/validator.go:228): 1 / 0 / <0 */
+/* aggSig.VerifyHash(mask.AggregatePublic, msg) with the resident aggregate (consensus/validator.go:228): 1 / 0 / <0 (HBLS_ERR_ARG
+ * for a null mask or signature).  Concurrent calls share turns (threading, above). */
 int  hbls_mask_verify(const hbls_mask* m, const uint8_t sig96[96], const void* msg, size_t msg_len);
 
 /* Running vote aggregate (SURVEY 8f.2; consensus/quorum/quorum.go:164-196 AggregateVotes re-deserialises every stored hex
@@ -285,7 +293,8 @@ int hbls_get_public_key_batch(size_t k, const uint8_t* sk32, uint8_t* pk48_out);
  * id -- hence the commit payload -- become known).  hbls_set_param("hm_cache", 0) turns the cache off.  0 ok. */
 int hbls_hash_prefetch(const void* msg, size_t msg_len);
 int hbls_hash_cache_stats(uint64_t* hits, uint64_t* misses);
-/* Part-1 calls combined so far (include/hbls.h: threading): turns run, requests served by them and the largest turn.  A process
+/* Part-1 calls, hbls_aggregate_verify and hbls_mask_verify combined so far (include/hbls.h: threading): turns run, requests served
+ * by them and the largest turn.  Calls refused for their arguments never join a turn and are not counted.  A process
  * whose herumi-API calls never overlap sees turns == requests and max_turn == 1.  Each pointer is nullable.  0 ok. */
 int hbls_coalesce_stats(uint64_t* turns, uint64_t* requests, uint64_t* max_turn);
 
