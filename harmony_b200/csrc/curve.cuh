@@ -314,6 +314,159 @@ template <class E> HB_DEV void g2_psi(jac<E>& r, const jac<E>& p) {
 template <class E> HB_DEV void g2_psi2(jac<E>& r, const jac<E>& p) {
     fp2_mul_fp(r.x, p.x, fp_k(K_PSI2_CX)); fp2_neg(r.y, p.y); r.z = p.z;
 }
+
+// ------------------------------------------------------------------ secret-scalar ladders (sign, GetPublicKey): constant time
+// The sequence of field operations, every branch and every address depend only on public data (the point, the item count), never on
+// the scalar: complete projective formulas (no identity / equal-point cases), a regular recoding whose digits are all non-zero, and
+// table reads that load every entry and keep one by select.
+// HB_CT_PROBE(tag) marks the formulas, the table reads and the ladder steps.  It compiles to nothing in the library; the constant-time
+// tests build with HB_CT_PROBE_HOST (host emulation: a trace of tags) or HB_CT_PROBE_DEVICE (active mask and count per thread) and
+// define hb_ct_probe themselves.
+#if defined(HB_CT_PROBE_HOST) || defined(HB_CT_PROBE_DEVICE)
+__device__ void hb_ct_probe(uint32_t tag);
+#define HB_CT_PROBE(tag) hb_ct_probe(tag)
+#else
+#define HB_CT_PROBE(tag) ((void)0)
+#endif
+enum { CT_ADD = 1, CT_DBL, CT_READ, CT_STEP, CT_GLS_STEP };
+
+template <class F> struct prj { F x, y, z; };     // homogeneous projective: (X/Z, Y/Z); identity (0 : 1 : 0)
+
+// 3b x by additions: b = 4 on G1 (12 x); b' = 4 (1 + i) on G2 (12 (1 + i) x, the helper of the Miller doubling step)
+HB_DEV void f_mul3b(fp& r, const fp& a) { fp t; fp_dbl(t, a); fp_add(t, t, a); fp_dbl(t, t); fp_dbl(r, t); }
+HB_DEV void f_mul3b(fp2& r, const fp2& a) { fp2_mul_twist3b(r, a); }
+HB_DEV void f_mul3b(fp2h& r, const fp2h& a) { fp2_mul_twist3b(r, a); }
+
+// complete addition for y^2 = x^3 + b (Renes-Costello-Batina 2016, Algorithm 7): 12 M + 2 (x 3b), valid for every pair of points
+// (the identity, P == Q, P == -Q included).  r may alias p or q.
+template <class F> HB_NOINLINE void prj_add(prj<F>& r, const prj<F>& p, const prj<F>& q) {
+    HB_CT_PROBE(CT_ADD);
+    F t0, t1, t2, t3, t4, x3, y3, z3;
+    f_mul(t0, p.x, q.x); f_mul(t1, p.y, q.y); f_mul(t2, p.z, q.z);
+    f_add(t3, p.x, p.y); f_add(t4, q.x, q.y); f_mul(t3, t3, t4);
+    f_add(t4, t0, t1); f_sub(t3, t3, t4);                                   // X1 Y2 + X2 Y1
+    f_add(t4, p.y, p.z); f_add(x3, q.y, q.z); f_mul(t4, t4, x3);
+    f_add(x3, t1, t2); f_sub(t4, t4, x3);                                   // Y1 Z2 + Y2 Z1
+    f_add(x3, p.x, p.z); f_add(y3, q.x, q.z); f_mul(x3, x3, y3);
+    f_add(y3, t0, t2); f_sub(y3, x3, y3);                                   // X1 Z2 + X2 Z1
+    f_dbl(x3, t0); f_add(t0, x3, t0);                                       // 3 X1 X2
+    f_mul3b(t2, t2);
+    f_add(z3, t1, t2); f_sub(t1, t1, t2);
+    f_mul3b(y3, y3);
+    f_mul(x3, t4, y3); f_mul(t2, t3, t1); f_sub(x3, t2, x3);
+    f_mul(y3, y3, t0); f_mul(t1, t1, z3); f_add(y3, t1, y3);
+    f_mul(t0, t0, t3); f_mul(z3, z3, t4); f_add(z3, z3, t0);
+    r.x = x3; r.y = y3; r.z = z3;
+}
+// complete doubling (Algorithm 9): 6 M + 2 S + 1 (x 3b)
+template <class F> HB_NOINLINE void prj_dbl(prj<F>& r, const prj<F>& p) {
+    HB_CT_PROBE(CT_DBL);
+    F t0, t1, t2, x3, y3, z3;
+    f_sqr(t0, p.y); f_dbl(z3, t0); f_dbl(z3, z3); f_dbl(z3, z3);           // 8 Y^2
+    f_mul(t1, p.y, p.z); f_sqr(t2, p.z);
+    f_mul3b(t2, t2);
+    f_mul(x3, t2, z3); f_add(y3, t0, t2);
+    f_mul(z3, t1, z3);
+    f_dbl(t1, t2); f_add(t2, t1, t2);
+    f_sub(t0, t0, t2); f_mul(y3, t0, y3); f_add(y3, x3, y3);
+    f_mul(t1, p.x, p.y); f_mul(x3, t0, t1); f_dbl(x3, x3);
+    r.x = x3; r.y = y3; r.z = z3;
+}
+template <class F> HB_DEV void prj_set_inf(prj<F>& r) { f_zero(r.x); f_one(r.y); f_zero(r.z); }
+// Jacobian (X/Z^2, Y/Z^3) -> (X Z : Y : Z^3); the all-zero identity -> (0 : 1 : 0).  Only for public points (the base of a ladder).
+template <class F> HB_DEV void prj_from_jac(prj<F>& r, const jac<F>& p) {
+    F z2, one; f_sqr(z2, p.z); f_mul(r.x, p.x, p.z); f_mul(r.z, z2, p.z); r.y = p.y;
+    f_one(one); f_cmov(r.y, one, pt_is_inf(p));
+}
+// (X : Y : Z) -> Jacobian (X Z, Y Z^2, Z) by products only; the identity (0 : Y : 0) lands on the all-zero struct
+template <class F> HB_DEV void prj_to_jac(jac<F>& r, const prj<F>& p) {
+    F z2; f_sqr(z2, p.z); f_mul(r.x, p.x, p.z); f_mul(r.y, p.y, z2); r.z = p.z;
+}
+template <class F> HB_DEV void pt_cmov(prj<F>& r, const prj<F>& a, bool c) { f_cmov(r.x, a.x, c); f_cmov(r.y, a.y, c); f_cmov(r.z, a.z, c); }
+// r = -r when c, by select
+template <class F> HB_DEV void pt_cneg_ct(prj<F>& r, bool c) { F n; f_neg(n, r.y); f_cmov(r.y, n, c); }
+// r = t[i]: every entry is read, the one wanted is kept by select (the index never forms an address)
+template <class F, int N> HB_DEV void pt_select_ct(prj<F>& r, const prj<F>* t, uint32_t i) {
+    HB_CT_PROBE(CT_READ);
+    r = t[0];
+#pragma unroll 1
+    for (int j = 1; j < N; j++) pt_cmov(r, t[j], (uint32_t)j == i);
+}
+
+// r = [k]p for any 256-bit k (8 little-endian 32-bit words), in constant time.  k is made odd (k' = k | 1) and recoded into 64 odd
+// signed digits of 4 bits, k' = sum_i d_i 16^i: d_i = ((bits 4i .. 4i+4 of k') | 1) - 16 for i < 63, d_63 = (k' >> 252) | 1 (the
+// recurrence k_{i+1} = (k_i - d_i) / 16 = (k_i >> 4) | 1).  Table of the odd multiples P, 3P, .., 15P; per window 4 doublings and one
+// addition of the selected, conditionally negated entry; the closing addition adds -P when k was even and the identity otherwise, so
+// k = 0 and k = r - 1 need no special case.  252 doublings + 64 additions + the table, whatever k.
+template <class F> HB_NOINLINE void pt_mul_ct(jac<F>& r, const jac<F>& p, const uint32_t* k) {
+    prj<F> P, T[8], acc, q;
+    prj_from_jac(P, p);
+    T[0] = P; prj_dbl(q, P);
+#pragma unroll 1
+    for (int j = 1; j < 8; j++) prj_add(T[j], T[j - 1], q);
+    const bool even = (k[0] & 1u) == 0;
+    uint32_t kk[9];
+    for (int j = 0; j < 8; j++) kk[j] = k[j];
+    kk[0] |= 1u; kk[8] = 0;
+    pt_select_ct<F, 8>(acc, T, ((kk[7] >> 28) | 1u) >> 1);                  // d_63 > 0: entry (d_63 - 1) / 2
+#pragma unroll 1
+    for (int i = 62; i >= 0; i--) {
+        HB_CT_PROBE(CT_STEP);
+        prj_dbl(acc, acc); prj_dbl(acc, acc); prj_dbl(acc, acc); prj_dbl(acc, acc);
+        const int b = 4 * i;
+        const uint32_t w = ((uint32_t)((((uint64_t)kk[(b >> 5) + 1] << 32) | kk[b >> 5]) >> (b & 31)) & 31u) | 1u;     // d_i + 16
+        const uint32_t neg = ((w >> 4) & 1u) ^ 1u;                           // d_i < 0
+        pt_select_ct<F, 8>(q, T, ((w ^ (15u * neg)) & 15u) >> 1);             // |d_i| = 2 entry + 1
+        pt_cneg_ct(q, neg != 0);
+        prj_add(acc, acc, q);
+    }
+    prj_set_inf(q);
+    prj<F> m = T[0]; pt_cneg_ct(m, true); pt_cmov(q, m, even);
+    prj_add(acc, acc, q);
+    prj_to_jac(r, acc);
+}
+
+// r = sk H on G2 from the base-Z digits of sk = d0 + d1 Z + d2 Z^2 + d3 Z^3 (d_j < Z = |z| < 2^64), in constant time.  psi acts as
+// [z] = [-Z], so sk H = d0 P0 + d1 P1 + d2 P2 + d3 P3 with P0 = H, P1 = -psi(H), P2 = psi^2(H), P3 = -psi^3(H).  Sign-aligned column
+// recoding (GLV-SAC, Faz-Hernandez, Longa, Sanchez 2014): with d0 odd, column i has the sign s_i = 2 bit_{i+1}(d0) - 1 (s_64 = +1) and
+// adds s_i (P0 + sum_j c_ij P_j), c_ij = the low bit of d_j after the earlier columns took theirs (d_j <- (d_j - s_i c_ij) / 2).  The
+// eight sums P0 + {0,1} P1 + {0,1} P2 + {0,1} P3 form the table; 65 columns of one doubling and one addition each.  d0 is made odd
+// (d0 | 1) and the closing addition adds -H when it was even, the identity otherwise.  h is the affine H (public); E = fp2 or fp2h.
+template <class E> HB_NOINLINE void g2_mul_gls_ct(jac<E>& r, const aff<E>& h, const uint64_t* d) {
+    jac<E> B[4];                                                              // P0..P3; every one has Z = 1, so it is its own
+    B[0].x = h.x; B[0].y = h.y; f_one(B[0].z);                                // projective form too
+    g2_psi(B[1], B[0]); pt_neg(B[1], B[1]);
+    g2_psi2(B[2], B[0]);
+    g2_psi(B[3], B[2]); pt_neg(B[3], B[3]);
+    prj<E> Pj[4], T[8], acc, q;
+    for (int j = 0; j < 4; j++) { Pj[j].x = B[j].x; Pj[j].y = B[j].y; Pj[j].z = B[j].z; }
+    T[0] = Pj[0];
+#pragma unroll 1
+    for (int u = 1; u < 8; u++) { const int top = u >= 4 ? 4 : u >= 2 ? 2 : 1; prj_add(T[u], T[u - top], Pj[top == 4 ? 3 : top]); }
+    const bool even = (d[0] & 1u) == 0;
+    uint64_t s = (d[0] | 1u) >> 1, k1 = d[1], k2 = d[2], k3 = d[3];
+    uint8_t col[65];                                                          // bits 0-2: table entry, bit 3: negative column
+#pragma unroll 1
+    for (int i = 0; i < 65; i++) {
+        const uint32_t pos = (uint32_t)(s & 1u) | (i == 64 ? 1u : 0u); s >>= 1;
+        const uint32_t c1 = (uint32_t)(k1 & 1u), c2 = (uint32_t)(k2 & 1u), c3 = (uint32_t)(k3 & 1u), ng = pos ^ 1u;
+        k1 = (k1 >> 1) + (c1 & ng); k2 = (k2 >> 1) + (c2 & ng); k3 = (k3 >> 1) + (c3 & ng);
+        col[i] = (uint8_t)(c1 | c2 << 1 | c3 << 2 | ng << 3);
+    }
+    prj_set_inf(acc);
+#pragma unroll 1
+    for (int i = 64; i >= 0; i--) {
+        HB_CT_PROBE(CT_GLS_STEP);
+        prj_dbl(acc, acc);
+        pt_select_ct<E, 8>(q, T, col[i] & 7u);
+        pt_cneg_ct(q, (col[i] >> 3) != 0);
+        prj_add(acc, acc, q);
+    }
+    prj_set_inf(q);
+    prj<E> m = Pj[0]; pt_cneg_ct(m, true); pt_cmov(q, m, even);
+    prj_add(acc, acc, q);
+    prj_to_jac(r, acc);
+}
 // Q in G2  <=>  psi(Q) == [z]Q   (same boolean as [r]Q == O; SURVEY A.5)
 template <class E> HB_NOINLINE bool g2_in_subgroup(const jac<E>& p) {
     if (pt_is_inf(p)) return true;

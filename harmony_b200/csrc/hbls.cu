@@ -16,6 +16,7 @@
 #include <vector>
 #include "../../include/hbls.h"
 #include "coalesce.hpp"
+#include "secret_key.hpp"
 #include "kernels.cuh"
 #include "device_forms.cuh"
 
@@ -587,25 +588,9 @@ void launch_exact_two_phase(size_t n, const g2a* sig, const g1a* pkneg, const g2
     LAUNCH(k_exact_publish, blocks_for(n, 256), 256, s, n, (const uint32_t*)nullptr, (const uint8_t*)verdict, d_results);
 }
 
-// sk (little-endian u64 x 4, < r < Z^4) -> its four base-Z digits, Z = |z| = 0xd201000000010000 (plain long division on the host)
-bool sk_digits_base_z(const uint64_t sk[4], uint64_t dig[4]) {
-    const uint64_t Z = 0xd201000000010000ull;
-    uint64_t v[4] = {sk[0], sk[1], sk[2], sk[3]};
-    for (int k = 0; k < 3; k++) {
-        unsigned __int128 rem = 0;
-        for (int i = 3; i >= 0; i--) { const unsigned __int128 cur = (rem << 64) | v[i]; v[i] = (uint64_t)(cur / Z); rem = cur % Z; }
-        dig[k] = (uint64_t)rem;
-    }
-    dig[3] = v[0];
-    return (v[1] | v[2] | v[3]) == 0;                 // always for sk < r < Z^4; a hand-filled struct >= Z^4 takes the plain ladder
-}
-
-// r (BLS12-381 group order), little-endian u64
-const uint64_t R_ORDER[4] = {0xffffffff00000001ull, 0x53bda402fffe5bfeull, 0x3339d80809a1d805ull, 0x73eda753299d7d48ull};
-bool scalar_lt_r(const uint64_t k[4]) {
-    for (int i = 3; i >= 0; i--) { if (k[i] < R_ORDER[i]) return true; if (k[i] > R_ORDER[i]) return false; }
-    return false;
-}
+// secret-key bytes on the host (secret_key.hpp): base-Z digits, the range check and equality in constant time, and wiping
+using hb_secret::sk_digits_base_z;
+using hb_secret::scalar_lt_r;
 
 // ------------------------------------------------------------------ herumi-API calls (part 1 of include/hbls.h), n requests at a
 // time.  Concurrent calls from different threads are combined into turns (coalesce.hpp); a turn stages the inputs of all its requests
@@ -653,14 +638,17 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     if (d_apk) na = nser = 0;
     size_t bm_bytes = 0;
     for (size_t i = 0; i < na; i++) bm_bytes += ver[i]->blen;
-    // signing keys in base |z| first (ladder over psi), hand-filled keys >= Z^4 after them (plain ladder)
+    // signing keys in base |z| first (ladder over psi), hand-filled structs >= Z^3 2^64 after them (256-bit ladder)
     std::vector<uint64_t> dig; size_t ngls = 0;
+    dig.reserve(4 * sgn.size());                        // no reallocation: a moved buffer would leave digits behind unwiped
+    struct WipeDigits { std::vector<uint64_t>& v; ~WipeDigits() { hb_secret::wipe(v.data(), v.size() * 8); } } wipe_dig{dig};
     {
         std::vector<Part1Req*> rest;
         for (Part1Req* r : sgn) {
             uint64_t d[4];
             if (sk_digits_base_z(static_cast<const blsSecretKey*>(r->a)->d, d)) { sgn[ngls++] = r; dig.insert(dig.end(), d, d + 4); }
             else rest.push_back(r);
+            hb_secret::wipe(d, sizeof d);
         }
         std::copy(rest.begin(), rest.end(), sgn.begin() + ngls);
     }
@@ -703,6 +691,10 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     g2a* hm = ar.take<g2a>(nh); uint8_t* ok_hm = ar.take<uint8_t>(nh);
     g2a* th = gather ? ar.take<g2a>(nk) : hm; uint8_t* tok = gather ? ar.take<uint8_t>(nk) : ok_hm;      // the H(m) table
     std::vector<uint8_t> hin(in.size), hout(out.size);
+    // the digit, key and GetPublicKey sections are adjacent: [key_lo, key_hi) holds every secret byte of the staging copy.  The host copy
+    // is wiped on every return path, the device copy on the stream after the ladder kernels.
+    const size_t key_lo = i_dig, key_hi = i_pub + np * 32;
+    struct WipeKeys { uint8_t* p; size_t n; ~WipeKeys() { hb_secret::wipe(p, n); } } wipe_keys{hin.data() + key_lo, key_hi - key_lo};
     for (size_t i = nser; i < nv && !d_apk; i++) memcpy(&hin[i_apk + i * sizeof(g1)], ver[i]->b, sizeof(g1));
     if (sig96) memcpy(&hin[i_sig], sig96, 96);
     else for (size_t i = nser; i < nv; i++) memcpy(&hin[i_sig + (i - nser) * sizeof(g2)], ver[i]->a, sizeof(g2));
@@ -764,6 +756,7 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     if (ngls) LAUNCH(k_sign_hm_gls_pair, blocks_for(2 * ngls, 32), 32, s, ngls, (const uint64_t*)(din + i_dig), hm + nv, (const uint8_t*)ok_hm + nv, (size_t)1, dsig_out, dsok);
     if (ns > ngls) LAUNCH(k_sign_hm_pair, blocks_for(2 * (ns - ngls), 32), 32, s, ns - ngls, (const uint8_t*)(din + i_sk), hm + nv + ngls, (const uint8_t*)ok_hm + nv + ngls,
                           (size_t)1, dsig_out + ngls, dsok + ngls);
+    if (ns || np) CK(cudaMemsetAsync(din + key_lo, 0, key_hi - key_lo, s));
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(hout.data(), dout, out.size, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -1092,10 +1085,12 @@ size_t blsSecretKeySerialize(void* buf, size_t maxBufSize, const blsSecretKey* s
 size_t blsSecretKeyDeserialize(blsSecretKey* sec, const void* buf, size_t bufSize) {
     if (bufSize < 32 || g.st_failed) return 0;
     uint64_t k[4]; memcpy(k, buf, 32);
-    if (!scalar_lt_r(k)) return 0;
-    memcpy(sec->d, k, 32); return 32;
+    const bool ok = scalar_lt_r(k);
+    if (ok) memcpy(sec->d, k, 32);
+    hb_secret::wipe(k, sizeof k);
+    return ok ? 32 : 0;
 }
-int blsSecretKeyIsEqual(const blsSecretKey* l, const blsSecretKey* r) { return !g.st_failed && memcmp(l, r, 32) == 0; }
+int blsSecretKeyIsEqual(const blsSecretKey* l, const blsSecretKey* r) { return !g.st_failed && hb_secret::eq32(l, r); }
 
 // ------------------------------------------------------------------ single-element group ops.  The herumi signatures of Add / Sub /
 // GetPublicKey are void: on a CUDA failure the destination becomes the identity and the error is kept for hbls_last_error().
@@ -1728,6 +1723,7 @@ static int sign_hash_batch_locked(size_t k, const uint8_t* sk32, const uint8_t* 
     CK(cudaMemcpyAsync(dsk, sk32, k * 32, cudaMemcpyHostToDevice, g.stream));
     if (msg_len) CK(cudaMemcpyAsync(dmsg, msgs, k * msg_len, cudaMemcpyHostToDevice, g.stream));
     LAUNCH(k_sign_hash, blocks_for(k, TPB), TPB, g.stream, k, dsk, dmsg, (uint32_t)msg_len, dpts, dok);
+    CK(cudaMemsetAsync(dsk, 0, k * 32, g.stream));                   // the keys leave the device with the ladder
     LAUNCH(k_g2_serialize, blocks_for(k, TPB), TPB, g.stream, k, dpts, dout);
     CK(cudaMemcpyAsync(sig96_out, dout, k * 96, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaMemcpyAsync(ok, dok, k, cudaMemcpyDeviceToHost, g.stream));
@@ -1746,6 +1742,7 @@ static int get_public_key_batch_locked(size_t k, const uint8_t* sk32, uint8_t* p
     uint8_t* dsk = ar.take<uint8_t>(k * 32); g1* dpts = ar.take<g1>(k); uint8_t* dout = ar.take<uint8_t>(k * 48);
     CK(cudaMemcpyAsync(dsk, sk32, k * 32, cudaMemcpyHostToDevice, g.stream));
     LAUNCH(k_g1_mul_gen, blocks_for(k, TPB), TPB, g.stream, k, dsk, dpts);
+    CK(cudaMemsetAsync(dsk, 0, k * 32, g.stream));
     LAUNCH(k_g1_serialize, blocks_for(k, TPB), TPB, g.stream, k, dpts, dout);
     CK(cudaMemcpyAsync(pk48_out, dout, k * 48, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));

@@ -1444,20 +1444,21 @@ __global__ void k_selftest_fp2h(uint32_t n, uint32_t seed, uint32_t* mismatches)
     }
 }
 
-// ---- scalar multiplication batches (R6 sign, R14 GetPublicKey)
+// ---- scalar multiplication batches (R6 sign, R14 GetPublicKey): constant-time ladders (curve.cuh pt_mul_ct, g2_mul_gls_ct).  Branches
+// here depend on public data only: the item count, whether H(m) exists.
 __global__ void k_g1_mul_gen(size_t n, const uint8_t* sk32, g1* out) {
     size_t i = HB_TID; if (i >= n) return;
     uint32_t k[8]; load_words(k, sk32 + 32 * i, 8);
-    g1 g, r; g1_generator(g); pt_mul(r, g, k, 8); out[i] = r;
+    g1 g, r; g1_generator(g); pt_mul_ct(r, g, k); out[i] = r;
 }
 __global__ void k_sign_hash(size_t n, const uint8_t* sk32, const uint8_t* msgs, uint32_t msg_len, g2* out, uint8_t* ok) {
     size_t i = HB_TID; if (i >= n) return;
     uint32_t k[8]; load_words(k, sk32 + 32 * i, 8);
     g2 h, r; bool good = map_to_g2(h, msgs + (size_t)msg_len * i, msg_len);
-    if (good) pt_mul(r, h, k, 8); else pt_set_inf(r);
+    if (good) pt_mul_ct(r, h, k); else pt_set_inf(r);
     out[i] = r; ok[i] = good ? 1 : 0;
 }
-// sigma = sk * H for an already-mapped H(m) (the library's H(m) cache, hbls.cu): one item per LANE PAIR, the 255-bit ladder on the
+// sigma = sk * H for an already-mapped H(m) (the library's H(m) cache, hbls.cu): one item per LANE PAIR, the 256-bit ladder on the
 // split carrier.  hm_stride = 0: every item signs the same point.  Output Jacobian (the layout of blsSignature).
 __global__ void k_sign_hm_pair(size_t n, const uint8_t* sk32, const g2a* hm, const uint8_t* ok_hm, size_t hm_stride, g2* out, uint8_t* ok) {
     const size_t i = HB_TID >> 1; if (i >= n) return;
@@ -1465,32 +1466,21 @@ __global__ void k_sign_hm_pair(size_t n, const uint8_t* sk32, const g2a* hm, con
     const g2a h = hm[i * hm_stride];
     const bool good = ok_hm[i * hm_stride] != 0 && !aff_is_inf(h);
     jac<fp2h> H, R; fp2h_pack(H.x, h.x); fp2h_pack(H.y, h.y); fp2_one(H.z);
-    pt_mul(R, H, k, 8);
+    pt_mul_ct(R, H, k);
     g2 r; fp2h_unpack(r.x, R.x); fp2h_unpack(r.y, R.y); fp2h_unpack(r.z, R.z);
     if (!good) pt_set_inf(r);
     if ((threadIdx.x & 1) == 0) { out[i] = r; ok[i] = good ? 1 : 0; }
 }
 // The same signature through the psi endomorphism (latency path of blsSignHash): the host writes sk = d0 + d1 Z + d2 Z^2 + d3 Z^3 in
 // base Z = |z| (four 64-bit digits: sk < r < Z^4); on G2 psi acts as [z] = [-Z], so  sk H = d0 H - d1 psi(H) + d2 psi^2(H) - d3 psi^3(H)
-// is ONE 64-step ladder over a 15-entry table of subset sums (64 doublings + <= 64 additions instead of 255 + 64 + 14).
+// is ONE 65-column ladder over an 8-entry table (g2_mul_gls_ct: 65 doublings + 66 additions instead of 252 + 64).
 __global__ void k_sign_hm_gls_pair(size_t n, const uint64_t* digits, const g2a* hm, const uint8_t* ok_hm, size_t hm_stride, g2* out, uint8_t* ok) {
     const size_t i = HB_TID >> 1; if (i >= n) return;
-    const uint64_t d0 = digits[4 * i], d1 = digits[4 * i + 1], d2 = digits[4 * i + 2], d3 = digits[4 * i + 3];
     const g2a h = hm[i * hm_stride];
     const bool good = ok_hm[i * hm_stride] != 0 && !aff_is_inf(h);
-    jac<fp2h> T[16], R;
-    pt_set_inf(T[0]);
-    fp2h_pack(T[1].x, h.x); fp2h_pack(T[1].y, h.y); fp2_one(T[1].z);          // H
-    g2_psi(T[2], T[1]); pt_neg(T[2], T[2]);                                    // -psi(H)
-    g2_psi2(T[4], T[1]);                                                       // psi^2(H)
-    g2_psi(T[8], T[4]); pt_neg(T[8], T[8]);                                    // -psi^3(H)
-    for (int m = 3; m < 16; m++) if (m & (m - 1)) pt_add(T[m], T[m & (m - 1)], T[m & -m]);
-    pt_set_inf(R);
-    for (int b = 63; b >= 0; b--) {
-        pt_dbl(R, R);
-        const int m = (int)((d0 >> b) & 1) | (int)((d1 >> b) & 1) << 1 | (int)((d2 >> b) & 1) << 2 | (int)((d3 >> b) & 1) << 3;
-        if (m) pt_add(R, R, T[m]);
-    }
+    aff<fp2h> H; fp2h_pack(H.x, h.x); fp2h_pack(H.y, h.y);
+    jac<fp2h> R;
+    g2_mul_gls_ct(R, H, digits + 4 * i);
     g2 r; fp2h_unpack(r.x, R.x); fp2h_unpack(r.y, R.y); fp2h_unpack(r.z, R.z);
     if (!good) pt_set_inf(r);
     if ((threadIdx.x & 1) == 0) { out[i] = r; ok[i] = good ? 1 : 0; }

@@ -43,6 +43,14 @@ extern "C" {
 #define HBLS_ERR_SELF_TEST (-4)     /* the self-test run at initialisation (HBLS_SELF_TEST=1) failed: the library refuses all work */
 
 /* ------------------------------------------------------------------ Part 1: herumi bls.h shape (SWAP_G) */
+/* Secret scalars.  blsSignHash, blsGetPublicKey, hbls_sign_hash_batch and hbls_get_public_key_batch multiply by the key in constant
+ * time: the sequence of field and group operations, every branch and every memory address depend only on public data (the message,
+ * whether it maps to a point, the item count), never on the key.  The ladders use complete projective formulas, a regular recoding
+ * with non-zero digits, and table reads that touch every entry; on the host, the base-|z| digits of the key, the range check of
+ * blsSecretKeyDeserialize and blsSecretKeyIsEqual take a fixed instruction sequence.  Key and digit bytes staged by the library are
+ * zeroed on the host before the call returns and on the device after the ladder kernels.  Not covered: H(m) and the verify-side
+ * scalars (public), the choice of ladder for a hand-filled struct >= |z|^3 2^64 (not a valid key), blsSecretKeySetByCSPRNG, and the
+ * caller's own copies of the key. */
 typedef struct { uint64_t d[4]; }  blsSecretKey;   /* 32 B: scalar < r, little-endian */
 typedef struct { uint64_t d[18]; } blsPublicKey;   /* 144 B: G1 Jacobian, Montgomery limbs; all-zero = identity */
 typedef struct { uint64_t d[36]; } blsSignature;   /* 288 B: G2 Jacobian, Montgomery limbs; all-zero = identity */
