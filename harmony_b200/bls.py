@@ -90,6 +90,7 @@ def lib():
         sig("hbls_verify_batch", c.c_int, sz, vp, vp, vp, sz, vp)
         sig("hbls_verify_batch_status", c.c_int, sz, vp, vp, vp, sz, vp)
         sig("hbls_sign_hash_batch", c.c_int, sz, vp, vp, sz, vp, vp)
+        sig("hbls_sign_hash_keys", c.c_int, sz, vp, sz, vp, sz, vp, vp, vp)
         sig("hbls_get_public_key_batch", c.c_int, sz, vp, vp)
         sig("hbls_map_to_g2", c.c_int, u8p, sz, vp)
         sig("hbls_fp_mul_batch", c.c_int, sz, vp, vp, vp)
@@ -459,6 +460,21 @@ def SignHashBatch(sks32: bytes, msgs: bytes, msg_len: int):
     rc = _need().hbls_sign_hash_batch(k, _buf(sks32), _buf(msgs), msg_len, out, ok)
     if rc != 0: raise HblsError(f"hbls_sign_hash_batch rc={rc}")
     return out.raw[:96 * k], ok.raw[:k]
+
+def SignHashKeys(sks32: bytes, msgs: bytes, msg_len: int, per_key=True, aggregate=True):
+    """hbls_sign_hash_keys: every one of the k keys in sks32 signs each of the m = len(msgs) // msg_len messages (a multi-key node's
+    votes: consensus/construct.go:97-114).  -> (sigs, aggs, ok): sigs = m*k signatures, key i on message j at (j*k + i)*96, or None
+    when per_key is False; aggs = m aggregates (what SignHash + Sign.Add over the keys + Serialize gives), or None when aggregate is
+    False; ok = m bytes, 0 where the message maps to no point (its signatures and aggregate are then 96 zero bytes)."""
+    if msg_len <= 0 or len(msgs) % msg_len: raise ValueError(f"msgs: {len(msgs)} bytes is not a whole number of {msg_len}-byte messages")
+    k = len(sks32) // 32
+    m = len(msgs) // msg_len
+    sigs = ctypes.create_string_buffer(max(96 * m * k, 1)) if per_key else None
+    aggs = ctypes.create_string_buffer(max(96 * m, 1)) if aggregate else None
+    ok = ctypes.create_string_buffer(max(m, 1))
+    rc = _need().hbls_sign_hash_keys(k, _buf(sks32), m, _buf(msgs), msg_len, sigs, aggs, ok)
+    if rc != 0: raise HblsError(f"hbls_sign_hash_keys rc={rc}")
+    return (sigs.raw[:96 * m * k] if per_key else None), (aggs.raw[:96 * m] if aggregate else None), ok.raw[:m]
 
 def HashPrefetch(msg: bytes):
     """Enqueue H(msg) into the library's device-resident H(m) cache and return at once (include/hbls.h: e.g. on ANNOUNCE, when the

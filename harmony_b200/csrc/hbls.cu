@@ -1736,6 +1736,115 @@ int hbls_sign_hash_batch(size_t k, const uint8_t* sk32, const uint8_t* msgs, siz
     std::lock_guard<std::mutex> lk(g.mu);
     return sign_hash_batch_locked(k, sk32, msgs, msg_len, sig96_out, ok);
 }
+
+// k keys sign each of m messages.  Every signature and aggregate is one ladder item.  Each message gets the per-key items of the keys
+// whose base-|z| digits fit, then its aggregate, whose key is the key sum mod r and always fits.  These run as one psi-ladder launch.
+// The per-key items of hand-filled keys >= Z^3 2^64 come after every message's items and take the 256-bit ladder.  H(m) is hashed or
+// fetched once per distinct message and shared by all of its items.
+static int sign_hash_keys_locked(size_t k, const uint8_t* sk32, size_t m, const uint8_t* msgs, size_t msg_len,
+                                 uint8_t* sigs96, uint8_t* aggs96, uint8_t* ok) {
+    cudaStream_t s = g.stream;
+    const bool per_key = sigs96 != nullptr, agg = aggs96 != nullptr;
+    // digits of each key (fitting keys) and of the key sum, at kd[4k..4k+4); wiped on every return path
+    std::vector<uint64_t> kd(4 * k + 4);
+    struct WipeDigits { std::vector<uint64_t>& v; ~WipeDigits() { hb_secret::wipe(v.data(), v.size() * 8); } } wipe_dig{kd};
+    std::vector<uint32_t> fit, big;                     // which keys take which ladder: public (only a hand-filled struct is big)
+    if (per_key) {
+        for (size_t i = 0; i < k; i++) {
+            uint64_t key[4]; memcpy(key, sk32 + 32 * i, 32);
+            (sk_digits_base_z(key, &kd[4 * i]) ? fit : big).push_back((uint32_t)i);
+            hb_secret::wipe(key, sizeof key);
+        }
+    }
+    if (agg) {
+        uint64_t sum[4];
+        hb_secret::sk_sum_mod_r(sk32, k, sum);
+        sk_digits_base_z(sum, &kd[4 * k]);              // sum < r: always fits
+        hb_secret::wipe(sum, sizeof sum);
+    }
+    const size_t nf = fit.size(), nb = big.size(), per_msg = nf + (agg ? 1 : 0);
+    const size_t ngls = m * per_msg, npair = m * nb, N = ngls + npair;
+    // H(m): one table entry per distinct message, misses at the front (one hash launch), cached entries at the back (as part1_locked)
+    std::vector<std::array<uint8_t, 48>> keys; std::vector<uint32_t> msg_entry(m);
+    {
+        std::map<std::array<uint8_t, 48>, uint32_t> seen;
+        for (size_t j = 0; j < m; j++) {
+            std::array<uint8_t, 48> key; hm_key(key.data(), msg_len ? msgs + j * msg_len : nullptr, msg_len);
+            auto it = seen.emplace(key, (uint32_t)keys.size());
+            if (it.second) keys.push_back(key);
+            msg_entry[j] = it.first->second;
+        }
+    }
+    const size_t nk = keys.size();
+    std::vector<uint32_t> pos(nk); std::vector<bool> cached(nk, false); size_t nmiss = 0;
+    for (size_t d = 0; d < nk; d++) cached[d] = hm_enabled() && hm_find(keys[d].data()) >= 0;
+    for (size_t d = 0, hit = 0; d < nk; d++) pos[d] = cached[d] ? (uint32_t)(nk - 1 - hit++) : (uint32_t)nmiss++;
+    // one distinct message: every item reads entry 0 (stride 0); else each item gets its message's point by k_broadcast_hm
+    const bool gather = nk > 1;
+    auto item_msg = [&](size_t i) { return i < ngls ? i / per_msg : (i - ngls) / nb; };
+    Layout in, out;
+    const size_t i_keys = in.put(nmiss * 48), i_idx = gather ? in.put(N * 4) : 0, i_dig = in.put(ngls * 32), i_sk = in.put(npair * 32);
+    const size_t o_ser = out.put(N * 96), o_ok = out.put(N);
+    Scratch* sc;
+    if (int e = reserve(s, in.size + out.size + (nk + (gather ? N : 0)) * (sizeof(g2a) + 1) + N * sizeof(g2) + 8 * 256, &sc)) return e;
+    Arena ar{sc->base, 0, sc->cap};
+    uint8_t* din = ar.take<uint8_t>(in.size); uint8_t* dout = ar.take<uint8_t>(out.size);
+    g2a* th = ar.take<g2a>(nk); uint8_t* tok = ar.take<uint8_t>(nk);
+    g2a* hm = gather ? ar.take<g2a>(N) : th; uint8_t* ok_hm = gather ? ar.take<uint8_t>(N) : tok;
+    g2* dsig = ar.take<g2>(N);
+    std::vector<uint8_t> hin(in.size), hout(out.size);
+    // the digit and key sections are adjacent: [key_lo, key_hi) holds every secret byte of the staging copy.  The host copy is wiped on
+    // every return path, the device copy on the stream after the ladder kernels.
+    const size_t key_lo = i_dig, key_hi = i_sk + npair * 32;
+    struct WipeKeys { uint8_t* p; size_t n; ~WipeKeys() { hb_secret::wipe(p, n); } } wipe_keys{hin.data() + key_lo, key_hi - key_lo};
+    for (size_t d = 0; d < nk; d++) if (!cached[d]) memcpy(&hin[i_keys + 48 * pos[d]], keys[d].data(), 48);
+    if (gather) for (size_t i = 0; i < N; i++) { const uint32_t e = pos[msg_entry[item_msg(i)]]; memcpy(&hin[i_idx + 4 * i], &e, 4); }
+    for (size_t j = 0; j < m; j++) {
+        uint8_t* dg = &hin[i_dig + 32 * j * per_msg];
+        for (size_t r = 0; r < nf; r++) memcpy(dg + 32 * r, &kd[4 * fit[r]], 32);
+        if (agg) memcpy(dg + 32 * nf, &kd[4 * k], 32);
+        for (size_t r = 0; r < nb; r++) memcpy(&hin[i_sk + 32 * (j * nb + r)], sk32 + 32 * big[r], 32);
+    }
+    CK(cudaMemcpyAsync(din, hin.data(), in.size, cudaMemcpyHostToDevice, s));
+    for (size_t d = 0; d < nk; d++) if (cached[d]) hm_fetch(keys[d].data(), th + pos[d], tok + pos[d], s);
+    if (hm_enabled()) g.hm_misses += nmiss;
+    if (nmiss) {
+        launch_hash_small(s, nmiss, din + i_keys, 48, th, tok);
+        if (hm_enabled()) for (size_t d = 0; d < nk; d++) if (!cached[d]) hm_store(keys[d].data(), th + pos[d], tok + pos[d], s);
+    }
+    if (gather) LAUNCH(k_broadcast_hm, blocks_for(N, 256), 256, s, N, (const uint32_t*)(din + i_idx), (const g2a*)th, (const uint8_t*)tok, hm, ok_hm);
+    const size_t stride = gather ? 1 : 0;
+    uint8_t* dok = dout + o_ok;
+    if (ngls) LAUNCH(k_sign_hm_gls_pair, blocks_for(2 * ngls, 32), 32, s, ngls, (const uint64_t*)(din + i_dig), (const g2a*)hm, (const uint8_t*)ok_hm, stride, dsig, dok);
+    if (npair) LAUNCH(k_sign_hm_pair, blocks_for(2 * npair, 32), 32, s, npair, (const uint8_t*)(din + i_sk), (const g2a*)hm + ngls * stride,
+                      (const uint8_t*)ok_hm + ngls * stride, stride, dsig + ngls, dok + ngls);
+    CK(cudaMemsetAsync(din + key_lo, 0, key_hi - key_lo, s));
+    LAUNCH(k_g2_serialize, blocks_for(N, TPB), TPB, s, N, (const g2*)dsig, dout + o_ser);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(hout.data(), dout, out.size, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (size_t i = 0; i < N; i++) {
+        const size_t j = item_msg(i);
+        uint8_t* dst = i >= ngls ? sigs96 + 96 * (j * k + big[(i - ngls) % nb])
+                     : i % per_msg < nf ? sigs96 + 96 * (j * k + fit[i % per_msg]) : aggs96 + 96 * j;
+        memcpy(dst, &hout[o_ser + 96 * i], 96);
+    }
+    for (size_t j = 0; j < m; j++) ok[j] = hout[o_ok + (per_msg ? j * per_msg : ngls + j * nb)] ? 1 : 0;
+    return 0;
+}
+int hbls_sign_hash_keys(size_t k, const uint8_t* sk32, size_t m, const uint8_t* msgs, size_t msg_len,
+                        uint8_t* sigs96, uint8_t* aggs96, uint8_t* ok) {
+    if (int e = ensure_init()) return e;
+    // every size the call forms: m (k + 1) items of staged, device and serialized bytes, k keys of 32 bytes, m messages of msg_len
+    size_t items = 0, bytes = 0, mbytes = 0;
+    const bool overflow = k + 1 == 0 || __builtin_mul_overflow(m, k + 1, &items)
+                          || __builtin_mul_overflow(items, (size_t)(96 + 32 + 4 + sizeof(g2) + sizeof(g2a) + 2), &bytes)
+                          || __builtin_mul_overflow(k, (size_t)32, &bytes) || __builtin_mul_overflow(m, msg_len, &mbytes);
+    if (k == 0 || (!sigs96 && !aggs96) || !sk32 || !ok || overflow || (!msgs && mbytes > 0)) return HBLS_ERR_ARG;
+    if (m == 0) return 0;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return sign_hash_keys_locked(k, sk32, m, msgs, msg_len, sigs96, aggs96, ok);
+}
 static int get_public_key_batch_locked(size_t k, const uint8_t* sk32, uint8_t* pk48_out) {
     Scratch* sc; if (int e = reserve(g.stream, k * (32 + sizeof(g1) + 48) + 4096, &sc)) return e;
     Arena ar{sc->base, 0, sc->cap};

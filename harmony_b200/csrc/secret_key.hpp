@@ -48,6 +48,38 @@ inline bool scalar_lt_r(const uint64_t k[4]) {
     return borrow != 0;
 }
 
+// v <- v - r when v >= r: the subtraction always runs and a mask made from its borrow selects the result
+inline void sub_r_if_ge(uint64_t v[4]) {
+    uint64_t t[4], borrow = 0;
+    for (int i = 0; i < 4; i++) {
+        const unsigned __int128 d = (unsigned __int128)v[i] - R_ORDER[i] - borrow;
+        t[i] = (uint64_t)d; borrow = (uint64_t)(d >> 64) & 1u;
+    }
+    const uint64_t keep = 0 - borrow;                               // all ones when v < r
+    for (int i = 0; i < 4; i++) v[i] = (v[i] & keep) | (t[i] & ~keep);
+    t[0] = t[1] = t[2] = t[3] = 0;
+    __asm__ __volatile__("" : : "r"(t) : "memory");
+}
+
+// sum = (sk_0 + ... + sk_{k-1}) mod r over k little-endian 32-byte keys.  Each key is first reduced by two conditional subtractions
+// (2^256 < 3r), so a hand-filled struct >= r adds what its own ladder signs with: sk H = (sk mod r) H.  acc + key < 2r < 2^256
+// never carries out of 256 bits, and one more conditional subtraction brings it back below r.
+inline void sk_sum_mod_r(const uint8_t* sk32, size_t k, uint64_t sum[4]) {
+    uint64_t acc[4] = {0, 0, 0, 0}, v[4];
+    for (size_t j = 0; j < k; j++) {
+        memcpy(v, sk32 + 32 * j, 32);
+        sub_r_if_ge(v); sub_r_if_ge(v);
+        uint64_t carry = 0;
+        for (int i = 0; i < 4; i++) {
+            const unsigned __int128 s = (unsigned __int128)acc[i] + v[i] + carry;
+            acc[i] = (uint64_t)s; carry = (uint64_t)(s >> 64);
+        }
+        sub_r_if_ge(acc);
+    }
+    for (int i = 0; i < 4; i++) { sum[i] = acc[i]; acc[i] = 0; v[i] = 0; }
+    __asm__ __volatile__("" : : "r"(acc), "r"(v) : "memory");
+}
+
 // 32-byte equality without an early exit
 inline bool eq32(const void* a, const void* b) {
     const uint8_t* x = static_cast<const uint8_t*>(a); const uint8_t* y = static_cast<const uint8_t*>(b);

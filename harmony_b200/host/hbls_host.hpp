@@ -309,6 +309,45 @@ struct PrivateKeys : std::vector<bls::PrivateKeyWrapper> {
         for (auto& k : *this) { if (seen.count(k.Pub->Bytes)) continue; seen.insert(k.Pub->Bytes); out.push_back(k); }
         return out;
     }
+    // The validator's vote payload (consensus/construct.go:97-114): sig := Sign{}; for each key { if s := SignHash(msg); s != nil {
+    // sig.Add(s) } }; sig.Serialize().  One hbls_sign_hash_keys call instead of k SignHash + k Add + one Serialize; a message that maps
+    // to no point gives the identity, 96 zero bytes, as the loop does.  Throws on a library error.
+    std::vector<uint8_t> SignHashAggregate(const std::vector<uint8_t>& msg) const {
+        std::vector<uint8_t> agg(96); uint8_t ok = 0;
+        if (empty()) return agg;                                        // no key: the loop never runs, Sign{} serialises to zeros
+        const std::vector<uint8_t> m = pad48(msg);
+        call(m, 1, nullptr, agg.data(), &ok);
+        return agg;
+    }
+    // The per-key loops (leader.go:57-75 and threshold.go:53-69: the leader's own votes; view_change_construct.go:402-483 and
+    // view_change.go:284: each key signs M1-or-NIL and the view id): out[j][i] = Serialize(key i's SignHash(msgs[j])), or an empty
+    // vector where SignHash returns nil.  Messages of any length: only their first 48 bytes enter the map, so each one is passed
+    // zero-padded (or cut) to 48 bytes.  Throws on a library error.
+    std::vector<std::vector<std::vector<uint8_t>>> SignHashEach(const std::vector<std::vector<uint8_t>>& msgs) const {
+        const size_t k = size(), m = msgs.size();
+        std::vector<std::vector<std::vector<uint8_t>>> out(m, std::vector<std::vector<uint8_t>>(k));
+        if (!k || !m) return out;
+        std::vector<uint8_t> blob;
+        for (auto& msg : msgs) { auto p = pad48(msg); blob.insert(blob.end(), p.begin(), p.end()); }
+        std::vector<uint8_t> sigs(96 * m * k), ok(m);
+        call(blob, m, sigs.data(), nullptr, ok.data());
+        for (size_t j = 0; j < m; j++)
+            if (ok[j]) for (size_t i = 0; i < k; i++) out[j][i].assign(sigs.begin() + 96 * (j * k + i), sigs.begin() + 96 * (j * k + i + 1));
+        return out;
+    }
+private:
+    static std::vector<uint8_t> pad48(const std::vector<uint8_t>& msg) {
+        std::vector<uint8_t> p(48, 0);
+        if (!msg.empty()) std::memcpy(p.data(), msg.data(), msg.size() < 48 ? msg.size() : 48);
+        return p;
+    }
+    void call(const std::vector<uint8_t>& msgs48, size_t m, uint8_t* sigs, uint8_t* aggs, uint8_t* ok) const {
+        std::vector<uint8_t> sk(32 * size());
+        for (size_t i = 0; i < size(); i++) std::memcpy(&sk[32 * i], (*this)[i].Pri->v.d, 32);
+        const int rc = hbls_sign_hash_keys(size(), sk.data(), m, msgs48.data(), 48, sigs, aggs, ok);
+        volatile uint8_t* w = sk.data(); for (size_t i = 0; i < sk.size(); i++) w[i] = 0;         // the staged key bytes
+        if (rc != 0) throw std::runtime_error("hbls_sign_hash_keys rc=" + std::to_string(rc));
+    }
 };
 inline PrivateKeys GetPrivateKeys(const std::vector<std::shared_ptr<bls_core::SecretKey>>& secretKeys) {
     PrivateKeys keys; for (auto& s : secretKeys) keys.push_back(bls::WrapperFromPrivateKey(s)); return keys;

@@ -17,7 +17,8 @@
  * GPU, or a batch call holds it, the calls that arrive queue up and the next caller in line runs them all as one turn
  * (hbls_coalesce_stats counts the turns).  VerifyHash and the two committee checks share one pairing launch and at most `coop_max`
  * of them go into one turn.  There is no timer or batching window: a call that finds the library idle runs at once, alone, with
- * the launches it has always made.  The batch entry points and the ballot box are not combined.  Device work is serialised by one library
+ * the launches it has always made.  The batch entry points (hbls_sign_hash_keys included) and the ballot box are not combined: they
+ * take the library mutex for the whole call.  Device work is serialised by one library
  * mutex and (except the *_device entry points on a caller stream) one library stream.  Scratch memory is per stream, so
  * asynchronous device-pointer calls on DIFFERENT streams do not share intermediates; calls on one stream are stream-ordered.
  * Messages: only the first min(len, 48) bytes enter the map to G2 (mcl setArrayMask; SURVEY A.3); batch entry points take the
@@ -43,11 +44,12 @@ extern "C" {
 #define HBLS_ERR_SELF_TEST (-4)     /* the self-test run at initialisation (HBLS_SELF_TEST=1) failed: the library refuses all work */
 
 /* ------------------------------------------------------------------ Part 1: herumi bls.h shape (SWAP_G) */
-/* Secret scalars.  blsSignHash, blsGetPublicKey, hbls_sign_hash_batch and hbls_get_public_key_batch multiply by the key in constant
- * time: the sequence of field and group operations, every branch and every memory address depend only on public data (the message,
- * whether it maps to a point, the item count), never on the key.  The ladders use complete projective formulas, a regular recoding
- * with non-zero digits, and table reads that touch every entry; on the host, the base-|z| digits of the key, the range check of
- * blsSecretKeyDeserialize and blsSecretKeyIsEqual take a fixed instruction sequence.  Key and digit bytes staged by the library are
+/* Secret scalars.  blsSignHash, blsGetPublicKey, hbls_sign_hash_batch, hbls_sign_hash_keys and hbls_get_public_key_batch multiply by
+ * the key in constant time: the sequence of field and group operations, every branch and every memory address depend only on public
+ * data (the message, whether it maps to a point, the item count), never on the key.  The ladders use complete projective formulas, a
+ * regular recoding with non-zero digits, and table reads that touch every entry; on the host, the base-|z| digits of the key, the key
+ * sum mod r of hbls_sign_hash_keys, the range check of blsSecretKeyDeserialize and blsSecretKeyIsEqual take a fixed instruction
+ * sequence.  Key and digit bytes staged by the library are
  * zeroed on the host before the call returns and on the device after the ladder kernels.  Not covered: H(m) and the verify-side
  * scalars (public), the choice of ladder for a hand-filled struct >= |z|^3 2^64 (not a valid key), blsSecretKeySetByCSPRNG, and the
  * caller's own copies of the key. */
@@ -291,10 +293,21 @@ int hbls_rlc_fold(size_t n_records, const uint8_t* records);
 /* batched SignHash / GetPublicKey (consensus/construct.go:97-114 with multibls keys) ; ok[j] = 1/0 */
 int hbls_sign_hash_batch(size_t k, const uint8_t* sk32, const uint8_t* msgs, size_t msg_len, uint8_t* sig96_out, uint8_t* ok);
 int hbls_get_public_key_batch(size_t k, const uint8_t* sk32, uint8_t* pk48_out);
+/* k keys sign each of m messages (consensus/construct.go:97-114, leader.go:57-75, threshold.go:53-69,
+ * view_change_construct.go:402-483).  sk32: k x 32 bytes (little-endian, as hbls_sign_hash_batch); msgs: m x msg_len bytes, the
+ * first min(msg_len, 48) of each enter the map.  sigs96 (nullable): m*k signatures, key i on message j at (j*k + i)*96.
+ * aggs96 (nullable): m aggregates, aggs96 + 96 j = sum over the k keys of their signatures on message j.  ok[j] = 1, or 0 when
+ * message j maps to no point: then its k signatures and its aggregate are 96 zero bytes (SignHash returns nil; the loop's Sign{}
+ * serialises to the identity).  0 ok; HBLS_ERR_ARG for k == 0, both outputs NULL, a NULL sk32 / ok, NULL msgs with m*msg_len > 0,
+ * or sizes whose products overflow; HBLS_ERR_CUDA.  m == 0 returns 0 and launches nothing.
+ * H(m) is hashed (or taken from the H(m) cache) once per distinct message, and every signature and aggregate of the call is one item
+ * of one ladder launch: an aggregate is (sum of the keys mod r) * H(m), since H(m) has order r, so its cost does not grow with k. */
+int hbls_sign_hash_keys(size_t k, const uint8_t* sk32, size_t m, const uint8_t* msgs, size_t msg_len,
+                        uint8_t* sigs96, uint8_t* aggs96, uint8_t* ok);
 
 /* H(m) cache.  The library keeps the hash-to-G2 points of the last 64 distinct messages on the device (LRU, keyed by the 48
- * zero-padded bytes the map reads).  blsSignHash, blsVerifyHash, hbls_aggregate_verify, hbls_mask_verify and the same-message form of
- * hbls_aggregate_verify_batch fill and consult it, so a validator that signs a block hash / commit payload (consensus/validator.go
+ * zero-padded bytes the map reads).  blsSignHash, hbls_sign_hash_keys, blsVerifyHash, hbls_aggregate_verify, hbls_mask_verify and the
+ * same-message form of hbls_aggregate_verify_batch fill and consult it, so a validator that signs a block hash / commit payload (consensus/validator.go
  * prepare / commit votes) finds H(m) ready when it verifies the PREPARED / COMMITTED aggregate over the same bytes
  * (validator.go:219-236) -- the reference's analogue is its LRU of decoded public keys (crypto/bls/mask.go:35-55).
  * hbls_hash_prefetch enqueues H(msg) on an auxiliary stream and returns at once (e.g. on ANNOUNCE, when block hash, number and view
