@@ -174,6 +174,17 @@ template <class F> HB_NOINLINE void pt_mul_zabs(jac<F>& r, const jac<F>& p) {
     }
     r = acc;
 }
+// the same ladder for an affine base: mixed additions (8 M + 3 S instead of 12 M + 4 S).  The all-zero encoding gives the identity,
+// acc == +-p takes pt_add_mixed's doubling / identity branches as pt_add's, so the result is the group element pt_mul_zabs gives.
+template <class F> HB_NOINLINE void pt_mul_zabs_aff(jac<F>& r, const aff<F>& p) {
+    jac<F> acc; pt_from_aff(acc, p);
+    for (int i = 62; i >= 0; i--) {
+        HB_USYNC();
+        pt_dbl(acc, acc);
+        if ((K_Z_ABS >> i) & 1) pt_add_mixed(acc, acc, p);
+    }
+    r = acc;
+}
 
 // r = [k]p for a 64-bit k (random-linear-combination coefficients): plain MSB-first double-and-add
 template <class F> HB_NOINLINE void pt_mul_u64(jac<F>& r, const jac<F>& p, uint64_t k) {
@@ -299,10 +310,10 @@ template <class E, int N, class Load> HB_NOINLINE void pt_mul_joint_naf(jac<E>& 
 HB_DEV void g1_generator(g1& r) { fp_set(r.x, K_G1_X); fp_set(r.y, K_G1_Y); fp_one(r.z); }
 
 // ------------------------------------------------------------------ endomorphisms and subgroup membership
-// psi(x, y) = (conj(x) * cx, conj(y) * cy): acts as [p] (== [z] on G2)
-HB_DEV void g2_psi_aff(g2a& r, const g2a& a) {
-    fp2 t; fp2_conj(t, a.x); fp2_mul(r.x, t, fp2_k(K_PSI_CX));
-    fp2_conj(t, a.y); fp2_mul(r.y, t, fp2_k(K_PSI_CY));
+// psi(x, y) = (conj(x) * cx, conj(y) * cy): acts as [p] (== [z] on G2); maps the all-zero identity to itself.  E = fp2 or fp2h.
+template <class E> HB_DEV void g2_psi_aff(aff<E>& r, const aff<E>& a) {
+    E t; fp2_conj(t, a.x); fp2_mul(r.x, t, fp2_k<E>(K_PSI_CX));
+    fp2_conj(t, a.y); fp2_mul(r.y, t, fp2_k<E>(K_PSI_CY));
 }
 // Jacobian form: psi(X, Y, Z) = (conj(X) cx, conj(Y) cy, conj(Z)) -- no inversion.  E = fp2 or the lane-pair carrier fp2h.
 template <class E> HB_DEV void g2_psi(jac<E>& r, const jac<E>& p) {
@@ -471,6 +482,13 @@ template <class E> HB_NOINLINE void g2_mul_gls_ct(jac<E>& r, const aff<E>& h, co
 template <class E> HB_NOINLINE bool g2_in_subgroup(const jac<E>& p) {
     if (pt_is_inf(p)) return true;
     jac<E> a, b; g2_psi(a, p); pt_mul_zabs(b, p); pt_neg(b, b);
+    return pt_eq(a, b);
+}
+// the same test of an affine point (the all-zero identity passes): the ladder adds its affine base with mixed additions
+template <class E> HB_NOINLINE bool g2_in_subgroup_aff(const aff<E>& p) {
+    if (aff_is_inf(p)) return true;
+    aff<E> q; g2_psi_aff(q, p);
+    jac<E> a, b; pt_from_aff(a, q); pt_mul_zabs_aff(b, p); pt_neg(b, b);
     return pt_eq(a, b);
 }
 // P in G1  <=>  phi(P) == -[z^2]P, phi(x, y) = (beta x, y)
@@ -666,6 +684,26 @@ template <class E> HB_NOINLINE void g2_clear_cofactor(jac<E>& r, const jac<E>& p
     pt_add(t2, zp, np); g2_psi(t2, t2);
     pt_dbl(t3, p); g2_psi2(t3, t3);
     pt_add(t1, t1, t2); pt_add(r, t1, t3);
+}
+// The same h(P) for an affine P, in the order of RFC 9380's clear_cofactor_bls12381_g2 (z < 0, so [z] = -[|z|]):
+//   t1 = [z]P,  t2 = [z](t1 + psi(P)),  h(P) = t2 - t1 - psi(P) - P + psi^2(2P)
+// (t2 = [z^2]P + psi([z]P), so this is the combination above), in two halves of one |z| ladder each so that each can run as a kernel
+// of its own.  Three Jacobian points live at most, and every addend that is affine (P in the first ladder, psi(P), P) goes in by a
+// mixed addition.  Same group element as g2_clear_cofactor for every point of E', torsion included (the group law's exceptional cases
+// take their branches); the Jacobian representative may differ.
+template <class E> HB_NOINLINE void g2_clear_cofactor_aff_z1(jac<E>& t1, const aff<E>& p) {
+    pt_mul_zabs_aff(t1, p); pt_neg(t1, t1);
+}
+// h(P) from t1 = [z]P (g2_clear_cofactor_aff_z1) and P
+template <class E> HB_NOINLINE void g2_clear_cofactor_aff_z2(jac<E>& r, const jac<E>& t1, const aff<E>& p) {
+    jac<E> t2, t; aff<E> q;
+    g2_psi_aff(q, p); pt_add_mixed(t2, t1, q);
+    pt_mul_zabs(t2, t2); pt_neg(t2, t2);
+    pt_neg(t, t1); pt_add(t2, t2, t);
+    f_neg(q.y, q.y); pt_add_mixed(t2, t2, q);
+    q = p; f_neg(q.y, q.y); pt_add_mixed(t2, t2, q);
+    pt_from_aff(t, p); pt_dbl(t, t); g2_psi2(t, t);
+    pt_add(r, t2, t);
 }
 HB_NOINLINE bool map_to_g2(g2& r, const uint8_t* msg, uint32_t len) {
     fp2 t; hash_to_fp(t.a, msg, len); fp_zero(t.b);

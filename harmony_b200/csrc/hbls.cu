@@ -203,7 +203,8 @@ void launch_hash_batch(cudaStream_t s, size_t B, const uint8_t* d_msgs, uint32_t
         LAUNCH(k_hash_sw, capped_blocks(B, g.tpsm_sw, TPB), TPB, s, B, d_msgs, msg_len, hm, ok_hm);
         if (g.hash_split >= 2) {        // three kernels: map | cofactor clearing (Jacobian, into the S buffer the scaling stage fills later) | affine
             const unsigned t = lockstep_cta(g.tpsm_cof);
-            LAUNCH(k_hash_cofactor_pair, capped_blocks(2 * B, t, t), t, s, B, (const g2a*)hm, (const uint8_t*)ok_hm, S);
+            LAUNCH(k_hash_cofactor_z1_pair, capped_blocks(2 * B, t, t), t, s, B, (const g2a*)hm, (const uint8_t*)ok_hm, S);
+            LAUNCH(k_hash_cofactor_z2_pair, capped_blocks(2 * B, t, t), t, s, B, (const g2a*)hm, (const uint8_t*)ok_hm, S);
             LAUNCH(k_g2_normalize_batch, heavy_blocks(B), TPB, s, B, (const g2*)S, hm);
         } else
             LAUNCH(k_hash_cofactor, heavy_blocks(B), TPB, s, B, hm, (const uint8_t*)ok_hm);
@@ -356,7 +357,8 @@ void launch_hash_grouped(cudaStream_t s, size_t k, const MsgGroups& m, const uin
     if (!pairs) {          // map, then cofactor clearing and affine conversion over all k slots (the identity beyond what the map wrote)
         LAUNCH(k_hash_keys_sw, capped_blocks(k, g.tpsm_sw, TPB), TPB, s, k, (const unsigned*)m.count, pair_hi, (const uint8_t*)m.keys, m.hm_d, m.ok_d);
         const unsigned t = lockstep_cta(g.tpsm_cof);
-        LAUNCH(k_hash_cofactor_pair, capped_blocks(2 * k, t, t), t, s, k, (const g2a*)m.hm_d, (const uint8_t*)m.ok_d, S);
+        LAUNCH(k_hash_cofactor_z1_pair, capped_blocks(2 * k, t, t), t, s, k, (const g2a*)m.hm_d, (const uint8_t*)m.ok_d, S);
+        LAUNCH(k_hash_cofactor_z2_pair, capped_blocks(2 * k, t, t), t, s, k, (const g2a*)m.hm_d, (const uint8_t*)m.ok_d, S);
         LAUNCH(k_g2_normalize_batch, heavy_blocks(k), TPB, s, k, (const g2*)S, m.hm_d);
     }
     const size_t cg = (long long)k < g.hash_coop_max ? k : (size_t)(g.hash_coop_max > 0 ? g.hash_coop_max : 1);
@@ -1017,7 +1019,8 @@ int hbls_init_device(int device) {
     g.hash_split = envll("HBLS_HASH_SPLIT", 2); g.tpsm_sw = envll("HBLS_TPSM_SW", 512);
     CK(cudaFuncSetAttribute(k_hash_sw, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_hash_cofactor, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
-    CK(cudaFuncSetAttribute(k_hash_cofactor_pair, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
+    CK(cudaFuncSetAttribute(k_hash_cofactor_z1_pair, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
+    CK(cudaFuncSetAttribute(k_hash_cofactor_z2_pair, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_g2_normalize_batch, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     g.ready = true;
     return self_test_at_init();

@@ -377,8 +377,8 @@ __global__ void __launch_bounds__(64, HB_SW_MINBLOCKS) k_hash_sw(size_t n, const
     for (size_t i0 = HB_TID; i0 < n; i0 += (size_t)HB_BATCH_K * HB_STRIDE) hash_sw_items(i0, n, n, msgs, msg_len, pts, ok);
 }
 // cofactor clearing alone, Jacobian result (no per-thread arrays of pending items: the frame is the group law's own temporaries), and
-// the shared-inversion affine conversion as its own small kernel.  hbls.cu runs the cofactor clearing as k_hash_cofactor_pair; this
-// one-thread form is the reference tests compare it with.
+// the shared-inversion affine conversion as its own small kernel.  hbls.cu runs the cofactor clearing as k_hash_cofactor_z1_pair + _z2_pair; this
+// one-thread form is the reference tests compare k_hash_cofactor_pair with.
 __global__ void k_hash_cofactor_jac(size_t n, const g2a* pts, const uint8_t* ok, g2* out) {
   for (size_t i = HB_TID; i < n; i += HB_STRIDE) {
     g2 h; pt_set_inf(h);
@@ -794,16 +794,13 @@ __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_g2_subgrou
         aff<fp2h> a; a.x.c = a4[role]; a.y.c = a4[2 + role];
         const bool in = ok_in[i] != 0;
         bool good = in;
-        if (good && !aff_is_inf(a)) {
-            jac<fp2h> q; q.x = a.x; q.y = a.y; fp2_one(q.z);
-            good = g2_in_subgroup(q);
-        }
+        if (good) good = g2_in_subgroup_aff(a);
         if (zero_bad && in && !good) { fp* o = reinterpret_cast<fp*>(&pts[i]); fp_zero(o[role]); fp_zero(o[2 + role]); }
         if (role == 0) ok_out[i] = good ? 1 : 0;
     });
 }
 // cofactor clearing of the SW map's output (k_hash_sw) into the Jacobian buffer k_g2_normalize_batch converts: k_hash_cofactor_jac
-// on the lane-pair carrier
+// on the lane-pair carrier, byte for byte.  hbls.cu runs k_hash_cofactor_z1_pair + _z2_pair below; this one is the reference tests compare them with.
 __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_hash_cofactor_pair(size_t n, const g2a* pts, const uint8_t* ok, g2* out) {
     const int role = threadIdx.x & 1;
     pair_sweep(n, [&](size_t i) {
@@ -814,6 +811,35 @@ __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_hash_cofac
             g2_clear_cofactor(h, a);
         }
         fp* o = reinterpret_cast<fp*>(&out[i]); o[role] = h.x.c; o[2 + role] = h.y.c; o[4 + role] = h.z.c;
+    });
+}
+// the cofactor clearing hbls.cu runs, g2_clear_cofactor_aff_z1 / _z2 on the lane-pair carrier as two kernels of one |z| ladder each
+// (each the size of k_g2_subgroup_pair, instead of one kernel holding both ladders, the combination and both group laws): the first
+// writes t1 = [z]P (the identity where ok is not set) into out, the second turns it into h(P) in place.  Together they give the same
+// affine H(m) as k_hash_cofactor_pair after k_g2_normalize_batch.  The map's outputs are never the identity; the all-zero encoding
+// with ok set gives the identity, as in k_hash_cofactor_pair.
+__global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_hash_cofactor_z1_pair(size_t n, const g2a* pts, const uint8_t* ok, g2* out) {
+    const int role = threadIdx.x & 1;
+    pair_sweep(n, [&](size_t i) {
+        jac<fp2h> t1; pt_set_inf(t1);
+        if (ok[i]) {
+            const fp* p4 = reinterpret_cast<const fp*>(&pts[i]);
+            aff<fp2h> a; a.x.c = p4[role]; a.y.c = p4[2 + role];
+            g2_clear_cofactor_aff_z1(t1, a);
+        }
+        fp* o = reinterpret_cast<fp*>(&out[i]); o[role] = t1.x.c; o[2 + role] = t1.y.c; o[4 + role] = t1.z.c;
+    });
+}
+__global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_hash_cofactor_z2_pair(size_t n, const g2a* pts, const uint8_t* ok, g2* io) {
+    const int role = threadIdx.x & 1;
+    pair_sweep(n, [&](size_t i) {
+        if (!ok[i]) return;
+        const fp* p4 = reinterpret_cast<const fp*>(&pts[i]);
+        aff<fp2h> a; a.x.c = p4[role]; a.y.c = p4[2 + role];
+        fp* o = reinterpret_cast<fp*>(&io[i]);
+        jac<fp2h> t1, h; t1.x.c = o[role]; t1.y.c = o[2 + role]; t1.z.c = o[4 + role];
+        g2_clear_cofactor_aff_z2(h, t1, a);
+        o[role] = h.x.c; o[2 + role] = h.y.c; o[4 + role] = h.z.c;
     });
 }
 __global__ void __launch_bounds__(32) k_pairing_coop2(size_t B, const fp2* f1, const uint8_t* irr1, const g1a* pk_neg, const g2a* hm,

@@ -13,7 +13,8 @@ ONLY="$*"
 cap k_rlc_accum_split 'k_rlc_accum_split' 270336
 cap k_rlc_lines_split 'k_rlc_lines_split' 270336
 cap k_hash_sw '^k_hash_sw$' 270336
-cap k_hash_cofactor_pair '^k_hash_cofactor_pair$' 270336
+cap k_hash_cofactor_z1_pair '^k_hash_cofactor_z1_pair$' 270336
+cap k_hash_cofactor_z2_pair '^k_hash_cofactor_z2_pair$' 270336
 cap k_g2_decode '^k_g2_decode$' 270336
 cap k_g2_subgroup_pair '^k_g2_subgroup_pair$' 270336
 cap k_rlc_scale_g1 '^k_rlc_scale_g1$' 270336
