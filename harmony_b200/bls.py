@@ -21,7 +21,7 @@ _COMPILED_TIME_VAR = 46
 PublicKeySizeInBytes = 48
 BLSSignatureSizeInBytes = 96
 
-ERR_CUDA, ERR_ARG, ERR_DECODE, ERR_SELF_TEST = -100, -2, -3, -4
+ERR_CUDA, ERR_ARG, ERR_DECODE, ERR_SELF_TEST, ERR_CAPTURE = -100, -2, -3, -4, -5
 
 _lib = None
 _inited = False
@@ -317,6 +317,19 @@ class Committee:
         if rc != 0: raise HblsError(f"hbls_verify_headers_device rc={rc}")
         return out
 
+    def AggregateVerifyBatchDevice(self, bitmaps, sigs, msgs, stream=None):
+        """hbls_aggregate_verify_batch_device on uint8 CUDA tensors bitmaps [B,blen], sigs [B,96], msgs [B,msg_len]: a new uint8
+        tensor [B] of 1 / 0 per round, filled asynchronously on `stream` (default: torch.cuda.current_stream())."""
+        L = _need()
+        B = _rows(sigs, "sigs", 96)
+        _rows(bitmaps, "bitmaps", self.blen(), B)
+        msg_len = _rows_any(msgs, "msgs", B)
+        st, out, h = _device_call(stream, B, (bitmaps, sigs, msgs))
+        if B == 0: return out
+        rc = L.hbls_aggregate_verify_batch_device(self.h, B, _ptr(bitmaps), self.blen(), _ptr(sigs), _ptr(msgs), msg_len, _ptr(out), h)
+        if rc != 0: raise HblsError(f"hbls_aggregate_verify_batch_device rc={rc}")
+        return out
+
 HDR_BAD_SIG, HDR_OK, HDR_NO_QUORUM, HDR_BAD_ENCODING = 0, 1, 2, 3
 
 def AggregateVerifyItems(committees, bitmaps, sigs96: bytes, msgs: bytes, msg_len: int) -> bytes:
@@ -436,6 +449,8 @@ def AggregateVerifyItemsDevice(committees, bitmaps, sigs, msgs, stream=None):
     st, out, h = _device_call(stream, k, (bitmaps, sigs, msgs))
     if k == 0: return out
     rc = L.hbls_aggregate_verify_items_device(k, arr, _ptr(bitmaps), _ptr(sigs), _ptr(msgs), msg_len, _ptr(out), h)
+    if rc == ERR_CAPTURE:
+        raise HblsError("hbls_aggregate_verify_items_device cannot be captured into a CUDA graph (HBLS_ERR_CAPTURE): nothing was enqueued")
     if rc != 0: raise HblsError(f"hbls_aggregate_verify_items_device rc={rc}")
     return out
 

@@ -48,11 +48,17 @@ HB_DEV bool grp_same(const uint8_t* msgs, uint32_t msg_len, size_t i, size_t j) 
 
 // open addressing over mask + 1 >= 2k slots (both arrays HB_GRP_EMPTY beforehand): item i claims the first slot of its probe
 // sequence that is empty or holds its key, and lowers that slot's representative to i.  A claimed slot is never released, so
-// every item of one key stops at the same slot.  (k0, k1): the call's hash key (slots, not results, depend on it).
-__global__ void k_group_insert(size_t k, const uint8_t* msgs, uint32_t msg_len, uint32_t mask, uint64_t k0, uint64_t k1, uint32_t* slot_item,
+// every item of one key stops at the same slot.  (k0, k1): the call's hash key (slots, not results, depend on it), by value (direct
+// calls: drawn on the host) or as grp_salt_dev pointers into device memory (captured calls: written by k_rlc_draw at every replay).
+struct grp_salt_dev { const uint64_t* p; };
+HB_DEV uint64_t grp_salt(uint64_t k) { return k; }
+HB_DEV uint64_t grp_salt(grp_salt_dev k) { return *k.p; }
+template <class K = uint64_t>
+__global__ void k_group_insert(size_t k, const uint8_t* msgs, uint32_t msg_len, uint32_t mask, K k0, K k1, uint32_t* slot_item,
                                uint32_t* slot_rep, uint32_t* item_slot) {
+  const uint64_t s0 = grp_salt(k0), s1 = grp_salt(k1);
   for (size_t i = HB_TID; i < k; i += HB_STRIDE) {
-    uint32_t s = (uint32_t)grp_hash(msgs, msg_len, i, k0, k1) & mask;
+    uint32_t s = (uint32_t)grp_hash(msgs, msg_len, i, s0, s1) & mask;
     for (;;) {
         const uint32_t prev = atomicCAS(&slot_item[s], HB_GRP_EMPTY, (uint32_t)i);
         if (prev == HB_GRP_EMPTY || grp_same(msgs, msg_len, prev, i)) { atomicMin(&slot_rep[s], (uint32_t)i); item_slot[i] = s; break; }

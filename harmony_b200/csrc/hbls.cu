@@ -17,6 +17,7 @@
 #include "../../include/hbls.h"
 #include "coalesce.hpp"
 #include "secret_key.hpp"
+#include "chacha20.hpp"
 #include "kernels.cuh"
 #include "device_forms.cuh"
 
@@ -69,6 +70,9 @@ struct Ctx {
                                                             // once the groups fill the chip, 2 always the joint ladder
     // coefficient stream: ChaCha20 keyed from /dev/urandom, block counter = call number
     uint32_t chacha_key[8] = {}; uint64_t rlc_calls = 0;
+    // the device's copy of that key and its draw counter (k_rlc_draw: calls captured into a CUDA graph draw at every replay), and the
+    // draw of the captured call being enqueued (nullptr outside one)
+    uint32_t* d_chacha_key = nullptr; unsigned long long* d_draws = nullptr; rlc_draw_out* cap_draw = nullptr;
     // last batch
     hbls_batch_info info = {}; Scratch* info_sc = nullptr; bool info_valid = false;
     // last error of a call that cannot return one
@@ -97,6 +101,16 @@ void note_error(cudaError_t e, const char* what, const char* file, int line) {
 }
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { note_error(e_, #call, __FILE__, __LINE__); return HBLS_ERR_CUDA; } } while (0)
 
+// The library's own host-side CUDA calls (allocation, synchronisation) run in relaxed capture mode: a caller's capture in global mode
+// on another thread would otherwise make them fail (cudaMalloc and cudaStreamSynchronize are "potentially unsafe" while it is open).
+// None of them touches a capturing stream.  HostLock = that mode + g.mu, for the entry points.
+struct RelaxedCapture {
+    cudaStreamCaptureMode prev = cudaStreamCaptureModeRelaxed;
+    RelaxedCapture() { cudaThreadExchangeStreamCaptureMode(&prev); }
+    ~RelaxedCapture() { cudaThreadExchangeStreamCaptureMode(&prev); }
+};
+struct HostLock { RelaxedCapture relaxed; std::lock_guard<std::mutex> lk{g.mu}; };
+
 int ensure_init() {
     if (g.st_failed) { fprintf(stderr, "[hbls] the self-test failed at initialisation: the library refuses all work\n"); return HBLS_ERR_SELF_TEST; }
     if (g.ready) return 0;
@@ -114,6 +128,7 @@ struct Arena {
 };
 // scratch of stream s, grown to `bytes` (growing frees the old block: cudaFree waits for the device, so no kernel still reads it)
 int reserve(cudaStream_t s, size_t bytes, Scratch** out) {
+    RelaxedCapture relaxed;
     Scratch& sc = g.scratch[s];
     bytes += 4096;
     if (bytes > sc.cap) {
@@ -213,18 +228,7 @@ void launch_hash_batch(cudaStream_t s, size_t B, const uint8_t* d_msgs, uint32_t
 }
 
 // ------------------------------------------------------------------ coefficient stream (host): ChaCha20 block function, RFC 8439
-void chacha20_block(const uint32_t key[8], uint64_t counter, uint32_t out[16], uint32_t block = 0) {
-    uint32_t st[16] = {0x61707865u, 0x3320646eu, 0x79622d32u, 0x6b206574u, key[0], key[1], key[2], key[3], key[4], key[5], key[6], key[7],
-                       (uint32_t)counter, (uint32_t)(counter >> 32), 0x68626c73u /* "hbls" */, block};
-    uint32_t x[16]; memcpy(x, st, sizeof x);
-    auto rotl = [](uint32_t v, int c) { return (v << c) | (v >> (32 - c)); };
-    auto qr = [&](int a, int b, int c, int d) {
-        x[a] += x[b]; x[d] ^= x[a]; x[d] = rotl(x[d], 16); x[c] += x[d]; x[b] ^= x[c]; x[b] = rotl(x[b], 12);
-        x[a] += x[b]; x[d] ^= x[a]; x[d] = rotl(x[d], 8);  x[c] += x[d]; x[b] ^= x[c]; x[b] = rotl(x[b], 7);
-    };
-    for (int r = 0; r < 10; r++) { qr(0, 4, 8, 12); qr(1, 5, 9, 13); qr(2, 6, 10, 14); qr(3, 7, 11, 15); qr(0, 5, 10, 15); qr(1, 6, 11, 12); qr(2, 7, 8, 13); qr(3, 4, 9, 14); }
-    for (int i = 0; i < 16; i++) out[i] = x[i] + st[i];
-}
+// (chacha20.hpp; calls captured into a CUDA graph draw from the same key on the device instead: kernels.cuh k_rlc_draw)
 // one fresh draw per position inside a group, per call (kernels.cuh: rlc_coeffs); the low bit of each half-scalar pair is forced
 // odd on the device (rlc_scale_pair), leaving 63 random bits per coefficient
 rlc_coeffs rlc_draw() {
@@ -308,7 +312,7 @@ VerifyBufs carve_verify(Arena& ar, size_t B) {
 // auxiliary streams while the caller's stream still aggregates the public keys (launch_verify_tail joins them before the pairing).
 static bool latency_path(size_t B);
 void fork_point(size_t B, Scratch* sc, cudaStream_t s) {
-    if (!latency_path(B) || !g.overlap || g.stage_timing) return;
+    if (!latency_path(B) || !g.overlap || g.stage_timing || g.cap_draw) return;      // a captured call stays on the caller's stream
     if (cudaEventRecord(sc->fork, s) == cudaSuccess) sc->forked = true;
 }
 // batched (random-linear-combination) form applies: default mode and a batch large enough
@@ -348,9 +352,14 @@ void launch_hash_grouped(cudaStream_t s, size_t k, const MsgGroups& m, const uin
                          uint8_t* ok_hm, g2* S) {
     cudaMemsetAsync(m.slot_item, 0xff, (size_t)(m.mask + 1) * 4, s);
     cudaMemsetAsync(m.slot_rep, 0xff, (size_t)(m.mask + 1) * 4, s);
-    uint32_t blk[16]; chacha20_block(g.chacha_key, ++g.rlc_calls, blk);          // the table's hash key: fresh per call, never seen outside
-    const uint64_t k0 = ((uint64_t)blk[1] << 32) | blk[0], k1 = ((uint64_t)blk[3] << 32) | blk[2];
-    LAUNCH(k_group_insert, blocks_for(k, 256), 256, s, k, d_msgs, msg_len, m.mask, k0, k1, m.slot_item, m.slot_rep, m.item_slot);
+    if (g.cap_draw)            // captured: the salt k_rlc_draw wrote for this replay
+        LAUNCH(k_group_insert, blocks_for(k, 256), 256, s, k, d_msgs, msg_len, m.mask, grp_salt_dev{&g.cap_draw->salt[0]}, grp_salt_dev{&g.cap_draw->salt[1]},
+               m.slot_item, m.slot_rep, m.item_slot);
+    else {
+        uint32_t blk[16]; chacha20_block(g.chacha_key, ++g.rlc_calls, blk);      // the table's hash key: fresh per call, never seen outside
+        const uint64_t k0 = ((uint64_t)blk[1] << 32) | blk[0], k1 = ((uint64_t)blk[3] << 32) | blk[2];
+        LAUNCH(k_group_insert, blocks_for(k, 256), 256, s, k, d_msgs, msg_len, m.mask, k0, k1, m.slot_item, m.slot_rep, m.item_slot);
+    }
     LAUNCH(k_group_compact, 1, HB_GRP_SCAN, s, k, d_msgs, msg_len, (const uint32_t*)m.slot_rep, (const uint32_t*)m.item_slot, m.pos, m.grp, m.keys, m.count);
     const unsigned long long coop_hi = (unsigned long long)g.hash_coop_max;
     const unsigned long long pair_hi = pairs ? (unsigned long long)k : (unsigned long long)(g.coop_max > g.hash_coop_max ? g.coop_max : g.hash_coop_max);
@@ -435,7 +444,8 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
         cudaStreamWaitEvent(s, sc->join[0], 0); cudaStreamWaitEvent(s, sc->join[1], 0);
     }
     STAGE_EV(4, sc, s);
-    hbls_batch_info& bi = g.info;
+    hbls_batch_info cap_info;                                  // a captured call leaves hbls_last_batch_info to the direct ones
+    hbls_batch_info& bi = g.cap_draw ? cap_info : g.info;
     bi = hbls_batch_info{}; bi.rounds = B; bi.mode = rlc ? 1 : 0;
     cudaMemsetAsync(v.counts, 0, 5 * sizeof(unsigned), s);
     if (rlc) {
@@ -443,32 +453,40 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
         // that still gives every SM a full CTA of lane pairs (fewer Miller-loop pairs and final exponentiations per round), else 4
         const size_t G = rlc_group_size(B);
         const size_t ng = B / G, nr = ng * G, tail = B - nr;
-        const rlc_coeffs co = rlc_draw();
         const bool full = 2 * ng >= (size_t)g.sm_count * HB_TPB_SPLIT;
         const unsigned pb = full ? split_blocks(2 * ng) : blocks_for(2 * ng, 64), pt = full ? HB_TPB_SPLIT : 64;
         const bool two_phase = g.rlc_two_phase && v.lines != nullptr && (full || g.rlc_two_phase >= 2);
         // blocks of HB_RLC_M groups: group g is member g / S of block g mod S; coefficients per (position, member)
         const bool blocks = rlc_blocks(ng, two_phase);
         const size_t S = blocks ? (((ng + HB_RLC_M - 1) / HB_RLC_M + 31) & ~(size_t)31) : 0;
-        const rlc_block_coeffs cb = blocks ? rlc_draw_block() : rlc_block_coeffs{};
         // blocks possible: the device picks the form from how the last such call ended (k_rlc_form); counts[2] / counts[3] gate the
         // group form's / block form's kernels, the scaling kernels take the matching coefficients
         const unsigned* blk_gate = blocks ? v.counts + 3 : nullptr;
-        if (blocks) LAUNCH(k_rlc_form, 1, 32, s, ng, g.rlc_block == 1 ? 1 : 0, (const int*)g.rlc_form, v.counts + 2);
         bool joint = false;
-        if (g.scale_split && HB_BATCH_INV) {
-            LAUNCH(k_rlc_scale_g1, capped_blocks(nr, g.tpsm_scale_g1, TPB), TPB, s, nr, ng, v.apk, co, v.pk_scaled, S, cb, blk_gate);
-            const unsigned t = lockstep_cta(g.tpsm_scale_g2);
-            // the joint ladder runs a lane pair per GROUP: G times fewer items than the per-round ladder, so it needs a full chip of groups
-            joint = g.scale_joint >= 2 || (g.scale_joint == 1 && full);
-            if (joint) {          // one ladder per group into the Jacobian Sg (the first ng entries of S), then the shared-inversion affine form
-                if (G == 8) LAUNCH(k_rlc_group_scale_g2_pair<8>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
-                else LAUNCH(k_rlc_group_scale_g2_pair<4>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
-                LAUNCH(k_g2_normalize_batch, heavy_blocks(ng), TPB, s, ng, (const g2*)v.S, v.Sg);
+        // the scaling stage with coefficients co / cb: drawn on the host (by value), or those k_rlc_draw wrote for this replay of a
+        // captured call (device pointers)
+        auto scale = [&](auto co, auto cb) {
+            if (blocks) LAUNCH(k_rlc_form, 1, 32, s, ng, g.rlc_block == 1 ? 1 : 0, (const int*)g.rlc_form, v.counts + 2);
+            if (g.scale_split && HB_BATCH_INV) {
+                LAUNCH(k_rlc_scale_g1, capped_blocks(nr, g.tpsm_scale_g1, TPB), TPB, s, nr, ng, v.apk, co, v.pk_scaled, S, cb, blk_gate);
+                const unsigned t = lockstep_cta(g.tpsm_scale_g2);
+                // the joint ladder runs a lane pair per GROUP: G times fewer items than the per-round ladder, so it needs a full chip of groups
+                joint = g.scale_joint >= 2 || (g.scale_joint == 1 && full);
+                if (joint) {          // one ladder per group into the Jacobian Sg (the first ng entries of S), then the shared-inversion affine form
+                    if (G == 8) LAUNCH(k_rlc_group_scale_g2_pair<8>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+                    else LAUNCH(k_rlc_group_scale_g2_pair<4>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+                    LAUNCH(k_g2_normalize_batch, heavy_blocks(ng), TPB, s, ng, (const g2*)v.S, v.Sg);
+                } else
+                    LAUNCH(k_rlc_scale_g2_pair, capped_blocks(2 * nr, t, t), t, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
             } else
-                LAUNCH(k_rlc_scale_g2_pair, capped_blocks(2 * nr, t, t), t, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
-        } else
-        LAUNCH(k_rlc_scale, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, (const uint64_t*)nullptr, v.pk_scaled, v.S, v.bad, S, cb, blk_gate);
+            LAUNCH(k_rlc_scale, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, (const uint64_t*)nullptr, v.pk_scaled, v.S, v.bad, S, cb, blk_gate);
+        };
+        if (g.cap_draw) scale(rlc_coeffs_dev{g.cap_draw->co.c}, rlc_block_coeffs_dev{g.cap_draw->cb.c});
+        else {
+            const rlc_coeffs co = rlc_draw();
+            const rlc_block_coeffs cb = blocks ? rlc_draw_block() : rlc_block_coeffs{};
+            scale(co, cb);
+        }
         if (!joint && G == 8) LAUNCH(k_rlc_group_sum<8>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
         else if (!joint) LAUNCH(k_rlc_group_sum<4>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
         STAGE_EV(5, sc, s);
@@ -569,6 +587,7 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
         bi.cta_threads = coop ? 32 : (full ? HB_TPB_SPLIT : 64);
     }
     STAGE_EV(6, sc, s);
+    if (g.cap_draw) return;                                    // captured: no host copy, no event, no batch info
     cudaMemcpyAsync(sc->h_counts, v.counts, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, s);
     cudaEventRecord(sc->done, s);
     g.info_sc = sc; g.info_valid = true;
@@ -784,6 +803,7 @@ int agg_verify_one_locked(Part1Req& r);       // a lone AGG request: the path of
 // runs r in a turn of the combiner (from any thread; the caller must not hold g.mu).  A turn of one AGG or MASK request runs the
 // launches its call made before it could be combined: the three-stream latency path of one round, or part1_locked on the mask's key.
 void part1_submit(Part1Req& r) {
+    RelaxedCapture relaxed;                  // whichever thread runs the turn synchronises g.stream
     g.part1.submit(r, g.mu,
         [](int kind) { return kind == RQ_VERIFY ? (size_t)(g.coop_max > 0 ? g.coop_max : 1) : PART1_CAP; },
         [](hbls_coalesce::Request** rq, size_t n) {
@@ -961,6 +981,48 @@ int set_mask_locked(hbls_mask* m, const uint8_t* bitmap) {
 void ensure_stage_events(Scratch* sc) {
     if (g.stage_timing && !sc->ev_ok) { for (int i = 0; i < 8; i++) cudaEventCreate(&sc->ev[i]); sc->ev_ok = true; }
 }
+// ------------------------------------------------------------------ device forms on a capturing stream (include/hbls.h).  The call
+// is enqueued into the caller's graph: its arena comes from cudaMallocAsync and goes back with cudaFreeAsync on the same stream (memory
+// nodes of that graph: every replay gets scratch of its own, shared with no direct call and no other graph, released with the graph);
+// k_rlc_draw writes the call's coefficients and grouping salt there at every replay.  Nothing else of the library is touched: no
+// g.scratch entry, no auxiliary stream, event, host copy or hbls_last_batch_info.
+// 1 when stream s is capturing, 0 when not, HBLS_ERR_CUDA
+int capturing(cudaStream_t s) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CK(cudaStreamIsCapturing(s, &cs));
+    return cs != cudaStreamCaptureStatusNone ? 1 : 0;
+}
+// body(sc, ar) enqueues the call's B rounds / items on s with the arena ar of `bytes`; sc is a stand-in that is never used while
+// g.cap_draw is set (no fork, no stage events, no counters)
+template <class F> int run_captured(cudaStream_t s, size_t bytes, size_t B, F body) {
+    bytes += sizeof(rlc_draw_out) + 256;
+    uint8_t* base = nullptr;
+    CK(cudaMallocAsync(reinterpret_cast<void**>(&base), bytes, s));
+    Arena ar{base, 0, bytes};
+    rlc_draw_out* draw = ar.take<rlc_draw_out>(1);
+    LAUNCH(k_rlc_draw, 1, 32, s, (const uint32_t*)g.d_chacha_key, g.d_draws, HB_RLC_DRAW_NONCE, rlc_applies(B) ? 18u : 2u, draw);
+    Scratch stand_in;
+    g.cap_draw = draw;
+    body(&stand_in, ar);
+    g.cap_draw = nullptr;
+    const cudaError_t launched = cudaGetLastError();
+    CK(cudaFreeAsync(base, s));
+    if (launched != cudaSuccess) { note_error(launched, "launch", __FILE__, __LINE__); return HBLS_ERR_CUDA; }
+    return 0;
+}
+// a device form's call: captured, or in the stream's arena (reserve) as it always was
+template <class F> int run_device_form(cudaStream_t s, size_t bytes, size_t B, F body) {
+    const int cap = capturing(s);
+    if (cap < 0) return cap;
+    if (cap) return run_captured(s, bytes, B, body);
+    Scratch* sc; if (int e = reserve(s, bytes, &sc)) return e;
+    ensure_stage_events(sc);
+    Arena ar{sc->base, 0, sc->cap};
+    body(sc, ar);
+    CK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 int self_test_at_init();      // selftest.cuh: HBLS_SELF_TEST=1 runs hbls_self_test here
@@ -968,7 +1030,7 @@ int self_test_at_init();      // selftest.cuh: HBLS_SELF_TEST=1 runs hbls_self_t
 extern "C" {
 
 int hbls_init_device(int device) {
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     if (g.st_failed) return HBLS_ERR_SELF_TEST;
     if (g.ready) return 0;
     int count = 0;
@@ -1005,11 +1067,14 @@ int hbls_init_device(int device) {
     CK(cudaFuncSetAttribute(k_pairing_verify_split_list, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_hash_to_g2, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_g2_decode, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
-    CK(cudaFuncSetAttribute(k_rlc_scale, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
+    CK(cudaFuncSetAttribute(k_rlc_scale<rlc_coeffs, rlc_block_coeffs>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
+    CK(cudaFuncSetAttribute(k_rlc_scale<rlc_coeffs_dev, rlc_block_coeffs_dev>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_mask_aggregate_serial, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaFuncSetAttribute(k_mask_aggregate, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     CK(cudaMalloc(&g.hm_slots, Ctx::HM_N * sizeof(g2a))); CK(cudaMalloc(&g.hm_ok, Ctx::HM_N));
     CK(cudaMalloc(&g.rlc_form, sizeof(int))); CK(cudaMemset(g.rlc_form, 0, sizeof(int)));
+    CK(cudaMalloc(&g.d_chacha_key, sizeof g.chacha_key)); CK(cudaMemcpy(g.d_chacha_key, g.chacha_key, sizeof g.chacha_key, cudaMemcpyHostToDevice));
+    CK(cudaMalloc(&g.d_draws, sizeof(unsigned long long))); CK(cudaMemset(g.d_draws, 0, sizeof(unsigned long long)));
     for (int i = 0; i < Ctx::HM_N; i++) {
         CK(cudaEventCreateWithFlags(&g.hm[i].filled, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&g.hm[i].read_done, cudaEventDisableTiming));
     }
@@ -1033,9 +1098,9 @@ int blsInit(int curve, int compiledTimeVar) {
 }
 uint64_t hbls_kernel_launch_count(void) { return g.launches.load(); }
 int hbls_build_info(void) { return (HB_BATCH_INV ? 1 : 0) | (HB_BATCH_K << 8); }
-int hbls_get_device(void) { if (int e = ensure_init()) return e; std::lock_guard<std::mutex> lk(g.mu); return g.device; }
-void hbls_set_batch_mode(int mode) { std::lock_guard<std::mutex> lk(g.mu); g.batch_mode = mode ? 1 : 0; }
-int hbls_get_batch_mode(void) { std::lock_guard<std::mutex> lk(g.mu); return g.batch_mode; }
+int hbls_get_device(void) { if (int e = ensure_init()) return e; HostLock lk; return g.device; }
+void hbls_set_batch_mode(int mode) { HostLock lk; g.batch_mode = mode ? 1 : 0; }
+int hbls_get_batch_mode(void) { HostLock lk; return g.batch_mode; }
 // tuning knobs by name (hbls_set_param); the self-test saves and restores all of them
 struct ParamDef { const char* name; long long Ctx::* slot; };
 const ParamDef PARAMS[] = {
@@ -1050,23 +1115,32 @@ static long long* param_slot(const char* name) {
     return nullptr;
 }
 int hbls_set_param(const char* name, long long value) {
-    std::lock_guard<std::mutex> lk(g.mu);
-    long long* p = param_slot(name);
+    HostLock lk;
+    long long* p = param_slot(name);          // "rlc_draws" is read-only: not in PARAMS
     if (!p || value < 0) return HBLS_ERR_ARG;
     if (p == &g.rlc_g && value != 0 && value != 4 && value != 8) return HBLS_ERR_ARG;
     if ((p == &g.rlc_block || p == &g.scale_joint) && value > 2) return HBLS_ERR_ARG;
     *p = value; return 0;
 }
-long long hbls_get_param(const char* name) { std::lock_guard<std::mutex> lk(g.mu); long long* p = param_slot(name); return p ? *p : -1; }
+long long hbls_get_param(const char* name) {
+    HostLock lk;
+    if (name && !strcmp(name, "rlc_draws")) {            // the device draw counter: waits for the device
+        unsigned long long d = 0;
+        if (!g.ready || cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(&d, g.d_draws, sizeof d, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+        return (long long)d;
+    }
+    long long* p = param_slot(name);
+    return p ? *p : -1;
+}
 int hbls_last_error(char* msg, size_t msg_cap) {
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     int e = g.last_err;
     if (msg && msg_cap) { strncpy(msg, g.last_err_msg, msg_cap - 1); msg[msg_cap - 1] = 0; }
     g.last_err = 0; g.last_err_msg[0] = 0;
     return e;
 }
 int hbls_last_batch_info(hbls_batch_info* out) {
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     if (!out || !g.info_valid || !g.info_sc) return HBLS_ERR_ARG;
     CK(cudaEventSynchronize(g.info_sc->done));
     *out = g.info;
@@ -1117,7 +1191,7 @@ int hbls_map_to_g2(const void* msg, size_t msg_len, uint8_t out96[96]) {
 // finds the point in the cache (stream-ordered after the fill).  0 ok (also when already cached or the cache is off).
 int hbls_hash_prefetch(const void* msg, size_t msg_len) {
     if (int e = ensure_init()) return e;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     if (!hm_enabled()) return 0;
     if (msg_len > 48) msg_len = 48;
     uint8_t key[48]; hm_key(key, msg, msg_len);
@@ -1141,7 +1215,7 @@ int hbls_coalesce_stats(uint64_t* turns, uint64_t* requests, uint64_t* max_turn)
     return 0;
 }
 int hbls_hash_cache_stats(uint64_t* hits, uint64_t* misses) {
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     if (hits) *hits = g.hm_hits;
     if (misses) *misses = g.hm_misses;
     return 0;
@@ -1204,10 +1278,10 @@ static int committee_create_locked(hbls_committee** out, const uint8_t* pk48, si
 int hbls_committee_create(hbls_committee** out, const uint8_t* pk48, size_t n, size_t* bad_index) {
     if (int e = ensure_init()) return e;
     if (!out) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return committee_create_locked(out, pk48, n, bad_index);
 }
-void hbls_committee_destroy(hbls_committee* c) { if (!c) return; std::lock_guard<std::mutex> lk(g.mu); cudaDeviceSynchronize(); delete c; }
+void hbls_committee_destroy(hbls_committee* c) { if (!c) return; HostLock lk; cudaDeviceSynchronize(); delete c; }
 size_t hbls_committee_size(const hbls_committee* c) { return c ? c->n : 0; }
 
 static int mask_aggregate_locked(const hbls_committee* c, const uint8_t* bitmap, size_t blen, uint8_t out_pk48[48]) {
@@ -1224,7 +1298,7 @@ static int mask_aggregate_locked(const hbls_committee* c, const uint8_t* bitmap,
 int hbls_mask_aggregate(const hbls_committee* c, const uint8_t* bitmap, size_t blen, uint8_t out_pk48[48]) {
     if (int e = ensure_init()) return e;
     if (!c || blen != ((c->n + 7) >> 3)) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return mask_aggregate_locked(c, bitmap, blen, out_pk48);
 }
 
@@ -1249,7 +1323,7 @@ static int aggregate_sigs_locked(const uint8_t* sig96, size_t n, uint8_t out96[9
 }
 int hbls_aggregate_sigs(const uint8_t* sig96, size_t n, uint8_t out96[96]) {
     if (int e = ensure_init()) return e;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return aggregate_sigs_locked(sig96, n, out96);
 }
 
@@ -1261,12 +1335,9 @@ int hbls_aggregate_verify_batch_device(const hbls_committee* c, size_t B, const 
     if (B == 0) return 0;
     std::lock_guard<std::mutex> lk(g.mu);
     cudaStream_t s = stream ? (cudaStream_t)stream : g.stream;
-    Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(B), &sc)) return e;
-    ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    int rc = agg_verify_device_locked(c, B, (const uint8_t*)d_bitmaps, blen, (const uint8_t*)d_sigs96, (const uint8_t*)d_msgs, msg_len, (uint8_t*)d_results, s, sc, ar, false);
-    CK(cudaGetLastError());
-    return rc;
+    return run_device_form(s, verify_scratch_bytes(B), B, [&](Scratch* sc, Arena& ar) {
+        agg_verify_device_locked(c, B, (const uint8_t*)d_bitmaps, blen, (const uint8_t*)d_sigs96, (const uint8_t*)d_msgs, msg_len, (uint8_t*)d_results, s, sc, ar, false);
+    });
 }
 // ------------------------------------------------------------------ bodies of the batch verifiers, shared by their host and device
 // forms: inputs in HBM, work enqueued on stream s in the scratch the caller reserved there, statuses computed on the device
@@ -1353,7 +1424,7 @@ int hbls_aggregate_verify_batch(const hbls_committee* c, size_t B, const uint8_t
     if (int e = ensure_init()) return e;
     if (!c || blen != ((c->n + 7) >> 3)) return HBLS_ERR_ARG;
     if (B == 0) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return agg_verify_host_locked(c, B, bitmaps, blen, sigs96, msgs, msg_len, results);
 }
 // a single check: a request of the Part-1 combiner (concurrent callers share turns; a lone call is agg_verify_one_locked)
@@ -1370,7 +1441,7 @@ int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96
     if (int e = ensure_init()) return e;
     if (!c || blen != ((c->n + 7) >> 3) || !status) return HBLS_ERR_ARG;        // DecodeSigBitmap: mask.SetMask length error (sig.go:43)
     if (n == 0) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return agg_verify_host_locked(c, n, bitmaps, blen, sigs96, payloads, payload_len, status, true, quorum);
 }
 
@@ -1397,7 +1468,7 @@ int hbls_aggregate_verify_items(size_t k, const hbls_committee* const* committee
     if (k == 0) return 0;
     if (!committees || !results) return HBLS_ERR_ARG;
     for (size_t j = 0; j < k; j++) if (!committees[j]) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return aggregate_verify_items_locked(k, committees, bitmaps, sigs96, msgs, msg_len, results);
 }
 
@@ -1420,14 +1491,14 @@ static int verify_batch_locked(size_t k, const uint8_t* pk48, const uint8_t* sig
 int hbls_verify_batch(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* results) {
     if (int e = ensure_init()) return e;
     if (k == 0) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return verify_batch_locked(k, pk48, sig96, msgs, msg_len, results, false);
 }
 int hbls_verify_batch_status(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* status) {
     if (int e = ensure_init()) return e;
     if (k == 0) return 0;
     if (!status) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return verify_batch_locked(k, pk48, sig96, msgs, msg_len, status, true);
 }
 
@@ -1436,13 +1507,10 @@ int hbls_verify_batch_status(size_t k, const uint8_t* pk48, const uint8_t* sig96
 // the H(m) cache is neither read nor filled: the host never sees the messages)
 static int verify_batch_status_device_locked(size_t k, const uint8_t* d_pk, const uint8_t* d_sig, const uint8_t* d_msgs, size_t msg_len,
                                              uint8_t* d_status, cudaStream_t s) {
-    Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(k) + group_bytes(k) + 2 * k + 4096, &sc)) return e;
-    ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    const MsgGroups mg = carve_groups(ar, k); uint8_t* dres = ar.take<uint8_t>(k);
-    verify_triples_body(k, d_pk, d_sig, d_msgs, msg_len, dres, d_status, s, sc, ar, false, &mg);
-    CK(cudaGetLastError());
-    return 0;
+    return run_device_form(s, verify_scratch_bytes(k) + group_bytes(k) + 2 * k + 4096, k, [&](Scratch* sc, Arena& ar) {
+        const MsgGroups mg = carve_groups(ar, k); uint8_t* dres = ar.take<uint8_t>(k);
+        verify_triples_body(k, d_pk, d_sig, d_msgs, msg_len, dres, d_status, s, sc, ar, false, &mg);
+    });
 }
 int hbls_verify_batch_status_device(size_t k, const void* d_pk48, const void* d_sig96, const void* d_msgs, size_t msg_len, void* d_status, void* stream) {
     if (int e = ensure_init()) return e;
@@ -1454,13 +1522,10 @@ int hbls_verify_batch_status_device(size_t k, const void* d_pk48, const void* d_
 }
 static int verify_headers_device_locked(const hbls_committee* c, size_t n, const uint8_t* d_sigs, const uint8_t* d_bitmaps, size_t blen,
                                         const uint8_t* d_payloads, size_t payload_len, size_t quorum, uint8_t* d_status, cudaStream_t s) {
-    Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(n) + group_bytes(n) + 2 * n + 4096, &sc)) return e;
-    ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    const MsgGroups mg = carve_groups(ar, n);
-    verify_headers_body(c, n, d_sigs, d_bitmaps, blen, d_payloads, payload_len, quorum, d_status, s, sc, ar, false, nullptr, &mg);
-    CK(cudaGetLastError());
-    return 0;
+    return run_device_form(s, verify_scratch_bytes(n) + group_bytes(n) + 2 * n + 4096, n, [&](Scratch* sc, Arena& ar) {
+        const MsgGroups mg = carve_groups(ar, n);
+        verify_headers_body(c, n, d_sigs, d_bitmaps, blen, d_payloads, payload_len, quorum, d_status, s, sc, ar, false, nullptr, &mg);
+    });
 }
 int hbls_verify_headers_device(const hbls_committee* c, size_t n, const void* d_sigs96, const void* d_bitmaps, size_t blen,
                                const void* d_payloads, size_t payload_len, size_t quorum, void* d_status, void* stream) {
@@ -1487,27 +1552,32 @@ int hbls_aggregate_verify_items_device(size_t k, const hbls_committee* const* co
     if (k == 0) return 0;
     if (!committees || !d_results) return HBLS_ERR_ARG;
     for (size_t j = 0; j < k; j++) if (!committees[j]) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    cudaStream_t s = stream ? (cudaStream_t)stream : g.stream;
+    HostLock lk;
+    // its descriptors come from a host array of handles that nothing would keep alive for a graph: refused before anything is
+    // enqueued or allocated, so the caller's capture stays valid
+    const int cap = capturing(s);
+    if (cap) return cap < 0 ? cap : HBLS_ERR_CAPTURE;
     return aggregate_verify_items_device_locked(k, committees, (const uint8_t*)d_bitmaps, (const uint8_t*)d_sigs96, (const uint8_t*)d_msgs, msg_len,
-                                                (uint8_t*)d_results, stream ? (cudaStream_t)stream : g.stream);
+                                                (uint8_t*)d_results, s);
 }
 
 // ------------------------------------------------------------------ persistent Mask / running vote aggregate (SURVEY 8f.2)
 int hbls_mask_create(hbls_mask** out, const hbls_committee* c) {
     if (int e = ensure_init()) return e;
     if (!out || !c) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     std::unique_ptr<hbls_mask> m(new hbls_mask); m->c = c; m->bitmap.assign((c->n + 7) >> 3, 0);
     CK(cudaMalloc(&m->d_acc, sizeof(g1)));
     CK(cudaMemsetAsync(m->d_acc, 0, sizeof(g1), g.stream));          // all-zero struct = identity (mask.go:88)
     CK(cudaStreamSynchronize(g.stream));
     *out = m.release(); return 0;
 }
-void hbls_mask_destroy(hbls_mask* m) { if (!m) return; std::lock_guard<std::mutex> lk(g.mu); cudaDeviceSynchronize(); delete m; }
+void hbls_mask_destroy(hbls_mask* m) { if (!m) return; HostLock lk; cudaDeviceSynchronize(); delete m; }
 int hbls_mask_clear(hbls_mask* m) {
     if (int e = ensure_init()) return e;
     if (!m) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     std::fill(m->bitmap.begin(), m->bitmap.end(), 0);
     CK(cudaMemsetAsync(m->d_acc, 0, sizeof(g1), g.stream));
     CK(cudaStreamSynchronize(g.stream));
@@ -1516,14 +1586,14 @@ int hbls_mask_clear(hbls_mask* m) {
 int hbls_mask_set_mask(hbls_mask* m, const uint8_t* bitmap, size_t blen) {
     if (int e = ensure_init()) return e;
     if (!m || blen != m->bitmap.size()) return HBLS_ERR_ARG;          // mask.go:114-120 "mismatching bitmap lengths"
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return set_mask_locked(m, bitmap);
 }
 // the read-modify-write of the bitmap stays under g.mu: concurrent callers that set different bits keep each other's bits
 int hbls_mask_set_bit(hbls_mask* m, size_t index, int enable) {
     if (int e = ensure_init()) return e;
     if (!m || index >= m->c->n) return HBLS_ERR_ARG;                   // mask.go:138-140 "index out of range"
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     std::vector<uint8_t> bm = m->bitmap;
     const uint8_t msk = (uint8_t)(1u << (index & 7));
     if (enable) bm[index >> 3] |= msk; else bm[index >> 3] &= (uint8_t)~msk;
@@ -1531,13 +1601,13 @@ int hbls_mask_set_bit(hbls_mask* m, size_t index, int enable) {
 }
 int hbls_mask_count_enabled(const hbls_mask* m) {
     if (!m) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return popcount_slots(m->bitmap.data(), m->c->n);
 }
 int hbls_mask_get(const hbls_mask* m, uint8_t* bitmap_out, size_t blen, uint8_t pk48_out[48]) {
     if (int e = ensure_init()) return e;
     if (!m || (bitmap_out && blen != m->bitmap.size())) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     if (bitmap_out) memcpy(bitmap_out, m->bitmap.data(), blen);
     if (pk48_out) {
         Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
@@ -1559,14 +1629,14 @@ int hbls_mask_verify(const hbls_mask* m, const uint8_t sig96[96], const void* ms
 int hbls_ballot_box_create(hbls_ballot_box** out, const hbls_committee* c) {
     if (int e = ensure_init()) return e;
     if (!out || !c) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     std::unique_ptr<hbls_ballot_box> b(new hbls_ballot_box); b->c = c; b->collected.assign((c->n + 7) >> 3, 0);
     CK(cudaMalloc(&b->d_sum, sizeof(g2)));
     CK(cudaMemsetAsync(b->d_sum, 0, sizeof(g2), g.stream));
     CK(cudaStreamSynchronize(g.stream));
     *out = b.release(); return 0;
 }
-void hbls_ballot_box_destroy(hbls_ballot_box* b) { if (!b) return; std::lock_guard<std::mutex> lk(g.mu); cudaDeviceSynchronize(); delete b; }
+void hbls_ballot_box_destroy(hbls_ballot_box* b) { if (!b) return; HostLock lk; cudaDeviceSynchronize(); delete b; }
 static int ballot_box_add_vote_locked(hbls_ballot_box* b, const uint8_t* signer_bitmap, size_t blen, const uint8_t sig96[96]) {
     const size_t n = b->c->n;
     for (size_t i = 0; i < n; i++)                                      // quorum.go:168-181: skip a ballot that shares a signer with a collected one
@@ -1586,7 +1656,7 @@ static int ballot_box_add_vote_locked(hbls_ballot_box* b, const uint8_t* signer_
 int hbls_ballot_box_add_vote(hbls_ballot_box* b, const uint8_t* signer_bitmap, size_t blen, const uint8_t sig96[96]) {
     if (int e = ensure_init()) return e;
     if (!b || !signer_bitmap || blen != b->collected.size()) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return ballot_box_add_vote_locked(b, signer_bitmap, blen, sig96);
 }
 static_assert(HB_BALLOT_ACCEPTED == HBLS_BALLOT_ACCEPTED && HB_BALLOT_COLLECTED == HBLS_BALLOT_COLLECTED &&
@@ -1625,7 +1695,7 @@ int hbls_ballot_box_submit_votes(hbls_ballot_box* b, size_t k, const uint8_t* si
     if (!b || !status || blen != b->collected.size() || msg_len > 64 || blen > HB_BALLOT_MAX_BYTES) return HBLS_ERR_ARG;
     if (k == 0) return 0;
     if (!signer_bitmaps || !sigs96 || (msg_len && !msg)) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return ballot_box_submit_votes_locked(b, k, signer_bitmaps, blen, sigs96, msg, msg_len, status);
 }
 static int ballot_box_aggregate_locked(const hbls_ballot_box* b, uint8_t out_sig96[96], uint8_t* bitmap_out, size_t blen) {
@@ -1641,7 +1711,7 @@ static int ballot_box_aggregate_locked(const hbls_ballot_box* b, uint8_t out_sig
 int hbls_ballot_box_aggregate(const hbls_ballot_box* b, uint8_t out_sig96[96], uint8_t* bitmap_out, size_t blen) {
     if (int e = ensure_init()) return e;
     if (!b || !out_sig96 || (bitmap_out && blen != b->collected.size())) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return ballot_box_aggregate_locked(b, out_sig96, bitmap_out, blen);
 }
 
@@ -1688,7 +1758,7 @@ static int rlc_partial_locked(size_t k, const uint8_t* pk48, const uint8_t* sig9
 int hbls_rlc_partial(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t record[HBLS_PARTIAL_BYTES]) {
     if (int e = ensure_init()) return e;
     if (!record) return HBLS_ERR_ARG;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return rlc_partial_locked(k, pk48, sig96, msgs, msg_len, record);
 }
 // the device part of hbls_rlc_fold (records that hold items and no undecodable one)
@@ -1714,7 +1784,7 @@ int hbls_rlc_fold(size_t n, const uint8_t* records) {
     size_t items = 0, bad = 0;
     for (size_t p = 0; p < n; p++) { PartialRecord r; memcpy(&r, records + p * HBLS_PARTIAL_BYTES, HBLS_PARTIAL_BYTES); items += r.n_items; bad += r.n_bad; }
     if (bad || items == 0) return 0;                                  // an undecodable / identity item somewhere, or nothing to prove: callers verify exactly
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return rlc_fold_locked(n, records);
 }
 
@@ -1736,7 +1806,7 @@ static int sign_hash_batch_locked(size_t k, const uint8_t* sk32, const uint8_t* 
 int hbls_sign_hash_batch(size_t k, const uint8_t* sk32, const uint8_t* msgs, size_t msg_len, uint8_t* sig96_out, uint8_t* ok) {
     if (int e = ensure_init()) return e;
     if (k == 0) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return sign_hash_batch_locked(k, sk32, msgs, msg_len, sig96_out, ok);
 }
 
@@ -1845,7 +1915,7 @@ int hbls_sign_hash_keys(size_t k, const uint8_t* sk32, size_t m, const uint8_t* 
                           || __builtin_mul_overflow(k, (size_t)32, &bytes) || __builtin_mul_overflow(m, msg_len, &mbytes);
     if (k == 0 || (!sigs96 && !aggs96) || !sk32 || !ok || overflow || (!msgs && mbytes > 0)) return HBLS_ERR_ARG;
     if (m == 0) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return sign_hash_keys_locked(k, sk32, m, msgs, msg_len, sigs96, aggs96, ok);
 }
 static int get_public_key_batch_locked(size_t k, const uint8_t* sk32, uint8_t* pk48_out) {
@@ -1863,7 +1933,7 @@ static int get_public_key_batch_locked(size_t k, const uint8_t* sk32, uint8_t* p
 int hbls_get_public_key_batch(size_t k, const uint8_t* sk32, uint8_t* pk48_out) {
     if (int e = ensure_init()) return e;
     if (k == 0) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return get_public_key_batch_locked(k, sk32, pk48_out);
 }
 
@@ -1881,16 +1951,16 @@ static int fp_mul_batch_locked(size_t n, const uint8_t* a48, const uint8_t* b48,
 int hbls_fp_mul_batch(size_t n, const uint8_t* a48, const uint8_t* b48, uint8_t* out48) {
     if (int e = ensure_init()) return e;
     if (n == 0) return 0;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return fp_mul_batch_locked(n, a48, b48, out48);
 }
 
 void hbls_stage_timing_enable(int on) {
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     g.stage_timing = on != 0; g.stage_sc = nullptr;
 }
 int hbls_stage_timing_get(float* ms_out, int max_stages) {
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     Scratch* sc = g.stage_sc;
     if (!sc || !sc->ev_ok) return 0;
     if (cudaEventSynchronize(sc->ev[6]) != cudaSuccess) return 0;
@@ -1912,12 +1982,12 @@ static int selftest_split_locked(uint32_t iters) {
 }
 int hbls_selftest_split(uint32_t iters) {
     if (int e = ensure_init()) return e;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     return selftest_split_locked(iters);
 }
 double hbls_probe_mac32_per_s(int iters, double* sm_clock_hz) {
     if (ensure_init()) return -1.0;
-    std::lock_guard<std::mutex> lk(g.mu);
+    HostLock lk;
     Scratch* sc; if (reserve(g.stream, 4096, &sc)) return -1.0;
     uint32_t* sink = reinterpret_cast<uint32_t*>(sc->base);
     unsigned long long* cyc = reinterpret_cast<unsigned long long*>(sc->base + 256);

@@ -898,20 +898,68 @@ struct rlc_coeffs { uint64_t c[HB_RLC_GMAX]; };
 // gets its own draw and only (0, 0) keeps 1.
 #define HB_RLC_M 16
 struct rlc_block_coeffs { uint64_t c[HB_RLC_GMAX][HB_RLC_M]; };
+// Coefficient sources of the scaling kernels (a template parameter of each, deduced at the launch): the structs above, passed by value
+// (direct calls: hbls.cu draws them on the host per call), or these pointer wrappers with the same c[k] / c[k][m] access into device
+// memory (calls captured into a CUDA graph: k_rlc_draw writes them there at every replay, so no coefficient is frozen into a node).
+struct rlc_coeffs_dev { const uint64_t* c; };
+struct rlc_block_coeffs_dev { const uint64_t (*c)[HB_RLC_M]; };
 // coefficient of round j = k ng + g: per position (S = 0: every group checked on its own), or per (position, block member)
-HB_DEV uint64_t rlc_coeff(const rlc_coeffs& co, size_t j, size_t ng, size_t S, const rlc_block_coeffs& cb) {
+template <class CO, class CB>
+HB_DEV uint64_t rlc_coeff(const CO& co, size_t j, size_t ng, size_t S, const CB& cb) {
     const size_t k = j / ng;
     if (!S) return k ? co.c[k] : 1ull;
     const size_t m = (j - k * ng) / S;
     return (k | m) ? cb.c[k][m] : 1ull;
 }
+// ---- secrets of a captured call, drawn on the device.  ChaCha20 block function (RFC 8439 section 2.3) on a whole 16-word state.
+HB_DEV uint32_t chacha_rotl(uint32_t v, int c) { return (v << c) | (v >> (32 - c)); }
+HB_DEV void chacha_qr(uint32_t* x, int a, int b, int c, int d) {
+    x[a] += x[b]; x[d] ^= x[a]; x[d] = chacha_rotl(x[d], 16); x[c] += x[d]; x[b] ^= x[c]; x[b] = chacha_rotl(x[b], 12);
+    x[a] += x[b]; x[d] ^= x[a]; x[d] = chacha_rotl(x[d], 8);  x[c] += x[d]; x[b] ^= x[c]; x[b] = chacha_rotl(x[b], 7);
+}
+HB_DEV void chacha20_block_dev(const uint32_t st[16], uint32_t out[16]) {
+    uint32_t x[16];
+    for (int i = 0; i < 16; i++) x[i] = st[i];
+    for (int r = 0; r < 10; r++) {
+        chacha_qr(x, 0, 4, 8, 12); chacha_qr(x, 1, 5, 9, 13); chacha_qr(x, 2, 6, 10, 14); chacha_qr(x, 3, 7, 11, 15);
+        chacha_qr(x, 0, 5, 10, 15); chacha_qr(x, 1, 6, 11, 12); chacha_qr(x, 2, 7, 8, 13); chacha_qr(x, 3, 4, 9, 14);
+    }
+    for (int i = 0; i < 16; i++) out[i] = x[i] + st[i];
+}
+// What k_rlc_draw writes into a captured call's scratch: keystream blocks 0 .. 17 of the call's counter, in order.  Block 0 = the
+// per-position coefficients, block 1 = the message-grouping salt (device_forms.cuh k_group_insert), blocks 2 .. 17 = the
+// per-(position, member) coefficients of the block form, each 64-bit value from two consecutive words as the host stream packs
+// them (hbls.cu rlc_draw, rlc_draw_block, launch_hash_grouped).
+struct rlc_draw_out { rlc_coeffs co; uint64_t salt[2]; uint64_t unused[6]; rlc_block_coeffs cb; };
+static_assert(sizeof(rlc_draw_out) == 18 * 64, "one keystream block per 64 bytes");
+// Words 12, 13 of the state are the call counter, 14 the stream's nonce word, 15 the block.  The host stream (hbls.cu chacha20_block)
+// uses the same key under nonce word 0x68626c73, so no keystream block is ever used by both.
+#define HB_RLC_DRAW_NONCE 0x68626c64u     /* "dlbh" */
+#ifndef HB_HOST_EMU
+// one warp: lane 0 takes the call's counter value (one atomicAdd on *draws, so every launch -- every graph replay -- draws anew), lane
+// b < nblocks writes block b.  The key is read from device memory and never appears in a kernel parameter or a graph node.
+__global__ void k_rlc_draw(const uint32_t* key, unsigned long long* draws, uint32_t nonce, uint32_t nblocks, rlc_draw_out* out) {
+    const unsigned lane = threadIdx.x;
+    unsigned long long call = 0;
+    if (lane == 0) call = atomicAdd(draws, 1ull);
+    call = __shfl_sync(0xffffffffu, call, 0);
+    if (lane >= nblocks) return;
+    uint32_t st[16] = {0x61707865u, 0x3320646eu, 0x79622d32u, 0x6b206574u, key[0], key[1], key[2], key[3], key[4], key[5], key[6], key[7],
+                       (uint32_t)call, (uint32_t)(call >> 32), nonce, lane};
+    uint32_t blk[16];
+    chacha20_block_dev(st, blk);
+    uint32_t* o = reinterpret_cast<uint32_t*>(out) + 16 * lane;
+    for (int i = 0; i < 16; i++) o[i] = blk[i];
+}
+#endif
 // per round: P_j = -r_j apk_j (affine), S_j = r_j sigma_j (Jacobian), bad_j
 #ifndef HB_SCALE_MINBLOCKS
 #define HB_SCALE_MINBLOCKS 1
 #endif
+template <class CO = rlc_coeffs, class CB = rlc_block_coeffs>
 __global__ void __launch_bounds__(64, HB_SCALE_MINBLOCKS) k_rlc_scale(size_t B, size_t ng, const g1* apk, const g2a* sig, const g2a* hm, const uint8_t* ok_sig, const uint8_t* ok_hm,
-                            const uint8_t* ok_pk, rlc_coeffs co, const uint64_t* per_item, g1a* pk_scaled_neg, g2* S, uint8_t* bad,
-                            size_t blk_stride = 0, rlc_block_coeffs cb = {}, const unsigned* blk_gate = nullptr) {
+                            const uint8_t* ok_pk, CO co, const uint64_t* per_item, g1a* pk_scaled_neg, g2* S, uint8_t* bad,
+                            size_t blk_stride = 0, CB cb = {}, const unsigned* blk_gate = nullptr) {
   if (blk_gate && *blk_gate == 0) blk_stride = 0;        // the device chose the group form (k_rlc_form): per-position coefficients
   // per_item (nullable): one independent coefficient per round -- needed when ALL rounds enter one combined check (the split of a
   // single batch over several GPUs, k_rlc_partial_coop); the grouped form shares co.c[position in group] across groups, the block
@@ -959,7 +1007,8 @@ __global__ void __launch_bounds__(64, HB_SCALE_MINBLOCKS) k_rlc_scale(size_t B, 
 }
 // the same stage as two kernels, one ladder each (hbls.cu "scale_split"): the G1 ladder (+ shared-inversion affine conversion) and the
 // G2 ladder are different code over different fields, and one kernel holding both stalls on instruction fetch
-__global__ void k_rlc_scale_g1(size_t B, size_t ng, const g1* apk, rlc_coeffs co, g1a* pk_scaled_neg, size_t blk_stride = 0, rlc_block_coeffs cb = {},
+template <class CO = rlc_coeffs, class CB = rlc_block_coeffs>
+__global__ void k_rlc_scale_g1(size_t B, size_t ng, const g1* apk, CO co, g1a* pk_scaled_neg, size_t blk_stride = 0, CB cb = {},
                                const unsigned* blk_gate = nullptr) {
   if (blk_gate && *blk_gate == 0) blk_stride = 0;
   for (size_t j0 = HB_TID; j0 < B; j0 += (size_t)HB_BATCH_K * HB_STRIDE) {
@@ -1003,9 +1052,10 @@ __global__ void __launch_bounds__(64, HB_SCALE_G2_MINBLOCKS) k_rlc_scale_g2(size
 }
 // k_rlc_scale_g2 on the lane-pair carrier (pair_sweep).  A warp's 16 pairs hold 16 consecutive rounds, which share their coefficient
 // (the 32 of a warp of the thread kernel do), so the JSF digits stay warp-uniform.
+template <class CO = rlc_coeffs, class CB = rlc_block_coeffs>
 __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_scale_g2_pair(size_t B, size_t ng, const g1* apk, const g2a* sig, const g2a* hm,
-                               const uint8_t* ok_sig, const uint8_t* ok_hm, const uint8_t* ok_pk, rlc_coeffs co, g2* S, uint8_t* bad,
-                               size_t blk_stride = 0, rlc_block_coeffs cb = {}, const unsigned* blk_gate = nullptr) {
+                               const uint8_t* ok_sig, const uint8_t* ok_hm, const uint8_t* ok_pk, CO co, g2* S, uint8_t* bad,
+                               size_t blk_stride = 0, CB cb = {}, const unsigned* blk_gate = nullptr) {
   if (blk_gate && *blk_gate == 0) blk_stride = 0;
   const int role = threadIdx.x & 1;
   pair_sweep(B, [&](size_t j) {
@@ -1035,9 +1085,10 @@ template <int G> __global__ void k_rlc_group_sum(size_t ngroups, const g2* S, g2
 // turns it affine) and the bad flag of each of the G rounds, by k_rlc_scale_g2_pair's rule.  A warp's 16 pairs hold 16 consecutive
 // groups, which share every coefficient (per position, or per (position, member) with the member stride a multiple of 32), so the
 // digits stay warp-uniform.
-template <int G> __global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_group_scale_g2_pair(size_t ng, const g1* apk, const g2a* sig,
-        const g2a* hm, const uint8_t* ok_sig, const uint8_t* ok_hm, const uint8_t* ok_pk, rlc_coeffs co, g2* Sg, uint8_t* bad,
-        size_t blk_stride = 0, rlc_block_coeffs cb = {}, const unsigned* blk_gate = nullptr) {
+template <int G, class CO = rlc_coeffs, class CB = rlc_block_coeffs>
+__global__ void __launch_bounds__(HB_TPB_SPLIT, HB_MINBLOCKS_SPLIT) k_rlc_group_scale_g2_pair(size_t ng, const g1* apk, const g2a* sig,
+        const g2a* hm, const uint8_t* ok_sig, const uint8_t* ok_hm, const uint8_t* ok_pk, CO co, g2* Sg, uint8_t* bad,
+        size_t blk_stride = 0, CB cb = {}, const unsigned* blk_gate = nullptr) {
   if (blk_gate && *blk_gate == 0) blk_stride = 0;
   const int role = threadIdx.x & 1;
   pair_sweep(ng, [&](size_t g) {

@@ -42,6 +42,7 @@ extern "C" {
 #define HBLS_ERR_ARG    (-2)        /* bad argument (e.g. bitmap length mismatch: mask.go:114-120) */
 #define HBLS_ERR_DECODE (-3)        /* an input failed to decode (not on curve / >= p / not in subgroup) */
 #define HBLS_ERR_SELF_TEST (-4)     /* the self-test run at initialisation (HBLS_SELF_TEST=1) failed: the library refuses all work */
+#define HBLS_ERR_CAPTURE (-5)       /* hbls_aggregate_verify_items_device on a stream that is capturing a CUDA graph (nothing enqueued) */
 
 /* ------------------------------------------------------------------ Part 1: herumi bls.h shape (SWAP_G) */
 /* Secret scalars.  blsSignHash, blsGetPublicKey, hbls_sign_hash_batch, hbls_sign_hash_keys and hbls_get_public_key_batch multiply by
@@ -164,10 +165,13 @@ int hbls_last_batch_info(hbls_batch_info* out);
  * exponentiation: 0 automatic, 1 forced on wherever they can run, 2 off; default from HBLS_RLC_BLOCK), "scale_joint" (signature scaling
  * as 0: a ladder per round + group sums, 1: one joint ladder per group when the groups fill the chip, 2: always the joint ladder;
  * default from HBLS_SCALE_JOINT).  Defaults come from HBLS_RLC_MIN, HBLS_RLC_G, HBLS_COOP_MAX,
- * HBLS_TPSM, HBLS_TPSM_SPLIT, HBLS_TPSM_LIGHT at blsInit.  0 ok, HBLS_ERR_ARG for an unknown name / bad value. */
+ * HBLS_TPSM, HBLS_TPSM_SPLIT, HBLS_TPSM_LIGHT at blsInit.  0 ok, HBLS_ERR_ARG for an unknown name / bad value.
+ * hbls_get_param("rlc_draws") reads the device draw counter of captured device-form calls (one draw per replay of each captured
+ * call, see the device forms below); it waits for the device first, and hbls_set_param refuses it (read-only). */
 int hbls_set_param(const char* name, long long value);
 long long hbls_get_param(const char* name);
-/* same, every pointer already in device memory (HBM); stream = cudaStream_t or NULL; asynchronous on that stream */
+/* same, every pointer already in device memory (HBM); stream = cudaStream_t or NULL; asynchronous on that stream.  It can be captured
+ * into a CUDA graph like the device forms below (same rules). */
 int hbls_aggregate_verify_batch_device(const hbls_committee* c, size_t B, const void* d_bitmaps, size_t blen,
                                        const void* d_sigs96, const void* d_msgs, size_t msg_len,
                                        void* d_results, void* stream);
@@ -223,7 +227,20 @@ int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96
  * Messages: items whose messages agree in the 48 zero-padded bytes the map reads are grouped on the device and each distinct
  * message is hashed to G2 once.  The H(m) cache is neither read nor filled (hbls_hash_cache_stats does not move).
  * The first call on a stream, or one larger than any before it there, allocates scratch (which may wait for the device); the items
- * form also waits, on the host, for the upload of the previous items call on the same stream if that has not run yet. */
+ * form also waits, on the host, for the upload of the previous items call on the same stream if that has not run yet.
+ * CUDA graphs: hbls_verify_batch_status_device, hbls_verify_headers_device and hbls_aggregate_verify_batch_device may be called on a
+ * stream that is capturing (cudaStreamBeginCapture, torch.cuda.graph), with no warm-up call.  The call then becomes part of the
+ * caller's graph: its scratch comes from cudaMallocAsync / cudaFreeAsync on that stream, so every replay gets scratch of its own
+ * (shared with no direct call and no other graph, released with the graph), and the random-linear-combination coefficients and the
+ * message-grouping salt are drawn on the device at every replay from the library's key (hbls_get_param("rlc_draws") grows by one per
+ * replay of each captured call; direct calls keep drawing on the host and leave it alone).  A captured call uses no library stream,
+ * allocates nothing outside the graph, does not synchronise, and leaves hbls_last_batch_info describing the last direct batch call.
+ * A graph keeps the batching regime (hbls_set_batch_mode) and the hbls_set_param values that held at capture, and the committee
+ * handle must outlive every graph that uses it.  hbls_kernel_launch_count counts the launches enqueued at capture, not replays.
+ * hbls_aggregate_verify_items_device cannot be captured (its descriptors come from the host array of handles): on a capturing stream
+ * it returns HBLS_ERR_CAPTURE before it enqueues or allocates anything, so the capture stays valid.
+ * The library's own synchronising calls (host forms, herumi-API calls, committee / mask / ballot-box calls) run in relaxed capture
+ * mode, so a global-mode capture held open by another thread does not make them fail. */
 int hbls_verify_batch_status_device(size_t k, const void* d_pk48, const void* d_sig96, const void* d_msgs, size_t msg_len,
                                     void* d_status, void* stream);
 int hbls_verify_headers_device(const hbls_committee* c, size_t n, const void* d_sigs96, const void* d_bitmaps, size_t blen,
@@ -324,7 +341,8 @@ int hbls_coalesce_stats(uint64_t* turns, uint64_t* requests, uint64_t* max_turn)
 int hbls_map_to_g2(const void* msg, size_t msg_len, uint8_t out96[96]);
 /* n field products on canonical little-endian 48-byte operands (kernel parity probe) */
 int hbls_fp_mul_batch(size_t n, const uint8_t* a48, const uint8_t* b48, uint8_t* out48);
-/* number of kernels this library has launched so far */
+/* number of kernels this library has launched so far (a call captured into a CUDA graph counts its launches once, at capture;
+ * replays of the graph do not count) */
 uint64_t hbls_kernel_launch_count(void);
 /* compile-time variant of the device code: bit 0 = shared inversions (Montgomery's trick over the items of a persistent thread in
  * hash-to-G2 and coefficient scaling), bits 8.. = items per shared inversion */
@@ -356,7 +374,8 @@ double hbls_probe_mac32_per_s(int iters, double* sm_clock_hz);
  * and restored afterwards.  Threading: the self-test holds the library mutex for its whole duration, so every other call waits.
  * It leaves the caller's state as it found it -- hbls_get_param values, the batch mode, stage timing and its recorded times,
  * hbls_last_batch_info, the H(m) cache (entries and hbls_hash_cache_stats), hbls_coalesce_stats -- except that
- * hbls_kernel_launch_count grows and the coefficient stream of the batched checks advances.
+ * hbls_kernel_launch_count grows and the coefficient streams of the batched checks advance (the host's, and the device draw
+ * counter hbls_get_param("rlc_draws"): one leg captures a small batched call into a graph and replays it).
  * With HBLS_SELF_TEST=1 in the environment, blsInit / hbls_init_device run it after initialising; when a leg fails they print the
  * failing legs on stderr and return HBLS_ERR_SELF_TEST, and from then on every call fails (later init calls too, without a rerun).
  * Returns 0 when every leg passes, the number of failed legs, or HBLS_ERR_CUDA on a runtime failure.  out (nullable). */
