@@ -84,6 +84,8 @@ def lib():
         sig("hbls_committee_size", sz, vp)
         sig("hbls_mask_aggregate", c.c_int, vp, u8p, sz, vp)
         sig("hbls_aggregate_sigs", c.c_int, u8p, sz, vp)
+        sig("hbls_aggregate_sigs_batch", c.c_int, sz, vp, vp, vp, vp)
+        sig("hbls_aggregate_sigs_batch_device", c.c_int, sz, sz, vp, vp, vp, vp, vp)
         sig("hbls_aggregate_verify", c.c_int, vp, u8p, sz, u8p, u8p, sz)
         sig("hbls_aggregate_verify_batch", c.c_int, vp, sz, vp, sz, vp, vp, sz, vp)
         sig("hbls_aggregate_verify_batch_device", c.c_int, vp, sz, vp, sz, vp, vp, sz, vp, vp)
@@ -358,6 +360,27 @@ def AggregateSigBytes(sigs96) -> bytes:
     if rc != 0: raise HblsError(f"hbls_aggregate_sigs rc={rc}")
     return out.raw
 
+# hbls_aggregate_sigs_batch statuses (include/hbls.h)
+AGG_OK, AGG_BAD_SIG_ENCODING, AGG_BAD_RANGE = 32, 33, 34
+
+def AggregateSigsBatch(sets):
+    """hbls_aggregate_sigs_batch: B AggregateSig calls in one device call.  sets = a list of lists of 96-byte signatures ->
+    (list of B 96-byte aggregates, list of B AGG_* statuses); a set with an undecodable signature gets AGG_BAD_SIG_ENCODING and the
+    identity's encoding, an empty set the identity with AGG_OK."""
+    B = len(sets)
+    if B == 0: return [], []
+    offsets = (ctypes.c_uint64 * (B + 1))()
+    blob = []
+    for j, s in enumerate(sets):
+        for sg in s:
+            if len(sg) != 96: raise ValueError(f"set {j}: a signature of {len(sg)} bytes, expected 96")
+            blob.append(bytes(sg))
+        offsets[j + 1] = len(blob)
+    out = ctypes.create_string_buffer(96 * B); st = ctypes.create_string_buffer(B)
+    rc = _need().hbls_aggregate_sigs_batch(B, offsets, b"".join(blob) or None, out, st)
+    if rc != 0: raise HblsError(f"hbls_aggregate_sigs_batch rc={rc}")
+    return [out.raw[96 * j:96 * j + 96] for j in range(B)], list(st.raw[:B])
+
 def VerifyBatch(pks48: bytes, sigs96: bytes, msgs: bytes, msg_len: int) -> bytes:
     k = len(sigs96) // 96
     res = ctypes.create_string_buffer(k if k else 1)
@@ -433,6 +456,25 @@ def VerifyBatchStatusDevice(pks, sigs, msgs, stream=None):
     rc = L.hbls_verify_batch_status_device(k, _ptr(pks), _ptr(sigs), _ptr(msgs), msg_len, _ptr(out), h)
     if rc != 0: raise HblsError(f"hbls_verify_batch_status_device rc={rc}")
     return out
+
+def AggregateSigsBatchDevice(offsets, sigs, stream=None):
+    """hbls_aggregate_sigs_batch_device: offsets = int64 CUDA tensor [B+1] (set j = rows offsets[j] .. offsets[j+1]-1), sigs [n,96]
+    -> (uint8 tensor [B,96] of aggregates, uint8 tensor [B] of AGG_* statuses), filled asynchronously on `stream` (default:
+    torch.cuda.current_stream()).  A reversed range or one past row n gives AGG_BAD_RANGE and the identity."""
+    import torch
+    L = _need()
+    n = _rows(sigs, "sigs", 96)
+    if not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1:
+        raise HblsError("offsets: expected a 1-D torch.int64 tensor of B+1 values")
+    if offsets.device != sigs.device or not offsets.is_contiguous(): raise HblsError(f"offsets: on {offsets.device}, expected {sigs.device}, contiguous")
+    B = int(offsets.numel()) - 1
+    st, status, h = _device_call(stream, B, (offsets, sigs))
+    with torch.cuda.stream(st):
+        out = torch.empty((B, 96), dtype=torch.uint8, device=sigs.device)
+    if B == 0: return out, status
+    rc = L.hbls_aggregate_sigs_batch_device(B, n, _ptr(offsets), _ptr(sigs), _ptr(out), _ptr(status), h)
+    if rc != 0: raise HblsError(f"hbls_aggregate_sigs_batch_device rc={rc}")
+    return out, status
 
 def AggregateVerifyItemsDevice(committees, bitmaps, sigs, msgs, stream=None):
     """hbls_aggregate_verify_items_device: item j = (committees[j], its bitmap, sigs[j], msgs[j]) -> uint8 tensor [k] of 1 / 0.

@@ -101,6 +101,9 @@ class DeviceBackend:
     def verify_headers(self, com, sigs96, bitmaps, msgs, quorum) -> bytes:
         return com.VerifyHeaders(b"".join(sigs96), b"".join(bitmaps), b"".join(_m48(m) for m in msgs), 48, quorum)
     def aggregate_sigs(self, sigs96) -> bytes: return bls.AggregateSigBytes(sigs96)
+    def aggregate_sigs_batch(self, sets):
+        """several AggregateSig calls at once: (aggregates, bls.AGG_* statuses)"""
+        return bls.AggregateSigsBatch(sets)
     def aggregate_keys(self, pks48) -> bytes:
         """sum of a multi-key vote's sender keys (consensus/leader.go:161-169): PublicKey.Add over the LRU-decoded keys"""
         acc = bls.PublicKey()
@@ -268,6 +271,19 @@ class viewChange:
         sigs = list(self.viewIDSigs.get(viewID, {}).values())
         if not sigs: return None, None
         return self.be.aggregate_sigs(sigs), bytes(self.viewIDBitmap[viewID])
+    def GetM2M3Bitmaps(self, viewID: int):
+        """(GetM2Bitmap(viewID), GetM3Bitmap(viewID)) -- the two aggregates the new leader puts into NEWVIEW back to back
+        (view_change_msg.go:119-120) -- from ONE batch call instead of two"""
+        tables = ((self.nilSigs, self.nilBitmap), (self.viewIDSigs, self.viewIDBitmap))
+        sets = [list(sigs.get(viewID, {}).values()) for sigs, _ in tables]
+        want = [j for j in range(2) if sets[j]]
+        out = [(None, None), (None, None)]
+        if want:
+            aggs, st = self.be.aggregate_sigs_batch([sets[j] for j in want])
+            for k, j in enumerate(want):
+                if st[k] != bls.AGG_OK: raise ValueError("err blsSignatureDeserialize")     # what AggregateSigBytes raises
+                out[j] = (aggs[k], bytes(tables[j][1][viewID]))
+        return out[0], out[1]
 
     # ---- a validator receiving NEWVIEW: ParseNewViewMessage (view_change_msg.go:191-250), VerifyNewViewMsg (:154-234), the M3 quorum
     # and the M1 proof of onNewView (view_change.go:470-500) -- up to three aggregate checks over messages of 8 / 1 / 32 bytes in ONE

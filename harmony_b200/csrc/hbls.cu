@@ -204,6 +204,16 @@ unsigned split_blocks(size_t nthreads) { return capped_blocks(nthreads, g.tpsm_s
 // lock-stepped lane-pair kernels: one CTA per SM, its size = the resident threads wanted for that kernel (multiple of 64, <= 512)
 unsigned lockstep_cta(long long t) { t = t < 64 ? 64 : (t > HB_TPB_SPLIT ? HB_TPB_SPLIT : t); return (unsigned)(t & ~63ll); }
 
+// signature decode of a large batch, one signature per thread: the subgroup test inside the decode, or (decode_split) as a
+// lane-pair kernel after it; a point outside G2 is zeroed and loses its ok flag either way
+void launch_g2_decode_checked(cudaStream_t s, size_t n, const uint8_t* d_sig96, g2a* pts, uint8_t* ok) {
+    if (g.decode_split) {
+        LAUNCH(k_g2_decode, capped_blocks(n, g.tpsm_dec, TPB), TPB, s, n, d_sig96, pts, ok, 0);
+        const unsigned t = lockstep_cta(g.tpsm_sub);
+        LAUNCH(k_g2_subgroup_pair, capped_blocks(2 * n, t, t), t, s, n, pts, (const uint8_t*)ok, ok, 1);
+    } else LAUNCH(k_g2_decode, capped_blocks(n, g.tpsm_dec, TPB), TPB, s, n, d_sig96, pts, ok, 1);
+}
+
 // hash-to-G2 of a small batch (latency path): one WARP per message while that still leaves every warp its own scheduler's worth of
 // an SM (the cofactor clearing runs as VM step programs), else one message per lane pair
 void launch_hash_small(cudaStream_t st, size_t n, const uint8_t* d_msgs, uint32_t msg_len, g2a* hm, uint8_t* ok_hm) {
@@ -408,11 +418,7 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
     // on the caller's stream, (B, sigma) after the decode on the decode stream with the signature's subgroup test beside it
     const bool warm = hit && split_ml;
     if (pairs) LAUNCH(k_g2_decode_pair, blocks_for(2 * B, 32), 32, sd, B, d_sig96, v.sig, v.ok_sig, warm ? 0 : 1);
-    else if (g.decode_split) {
-        LAUNCH(k_g2_decode, capped_blocks(B, g.tpsm_dec, TPB), TPB, s, B, d_sig96, v.sig, v.ok_sig, 0);
-        const unsigned t = lockstep_cta(g.tpsm_sub);
-        LAUNCH(k_g2_subgroup_pair, capped_blocks(2 * B, t, t), t, s, B, v.sig, (const uint8_t*)v.ok_sig, v.ok_sig, 1);
-    } else LAUNCH(k_g2_decode, capped_blocks(B, g.tpsm_dec, TPB), TPB, s, B, d_sig96, v.sig, v.ok_sig, 1);
+    else launch_g2_decode_checked(s, B, d_sig96, v.sig, v.ok_sig);
     if (warm) {
         cudaEventRecord(sc->mid, sd);
         LAUNCH(k_miller_pq_coop, coop_grid, 32, sd, B, (const g1a*)nullptr, v.sig, v.ok_sig, v.f1, v.irr1);
@@ -993,16 +999,20 @@ int capturing(cudaStream_t s) {
     return cs != cudaStreamCaptureStatusNone ? 1 : 0;
 }
 // body(sc, ar) enqueues the call's B rounds / items on s with the arena ar of `bytes`; sc is a stand-in that is never used while
-// g.cap_draw is set (no fork, no stage events, no counters)
-template <class F> int run_captured(cudaStream_t s, size_t bytes, size_t B, F body) {
+// g.cap_draw is set (no fork, no stage events, no counters).  draw = false: the call uses no coefficients (g.cap_draw stays null,
+// rlc_draws does not move), and its body touches no Scratch state either.
+template <class F> int run_captured(cudaStream_t s, size_t bytes, size_t B, F body, bool draw = true) {
     bytes += sizeof(rlc_draw_out) + 256;
     uint8_t* base = nullptr;
     CK(cudaMallocAsync(reinterpret_cast<void**>(&base), bytes, s));
     Arena ar{base, 0, bytes};
-    rlc_draw_out* draw = ar.take<rlc_draw_out>(1);
-    LAUNCH(k_rlc_draw, 1, 32, s, (const uint32_t*)g.d_chacha_key, g.d_draws, HB_RLC_DRAW_NONCE, rlc_applies(B) ? 18u : 2u, draw);
+    rlc_draw_out* drawn = nullptr;
+    if (draw) {
+        drawn = ar.take<rlc_draw_out>(1);
+        LAUNCH(k_rlc_draw, 1, 32, s, (const uint32_t*)g.d_chacha_key, g.d_draws, HB_RLC_DRAW_NONCE, rlc_applies(B) ? 18u : 2u, drawn);
+    }
     Scratch stand_in;
-    g.cap_draw = draw;
+    g.cap_draw = drawn;
     body(&stand_in, ar);
     g.cap_draw = nullptr;
     const cudaError_t launched = cudaGetLastError();
@@ -1011,10 +1021,10 @@ template <class F> int run_captured(cudaStream_t s, size_t bytes, size_t B, F bo
     return 0;
 }
 // a device form's call: captured, or in the stream's arena (reserve) as it always was
-template <class F> int run_device_form(cudaStream_t s, size_t bytes, size_t B, F body) {
+template <class F> int run_device_form(cudaStream_t s, size_t bytes, size_t B, F body, bool draw = true) {
     const int cap = capturing(s);
     if (cap < 0) return cap;
-    if (cap) return run_captured(s, bytes, B, body);
+    if (cap) return run_captured(s, bytes, B, body, draw);
     Scratch* sc; if (int e = reserve(s, bytes, &sc)) return e;
     ensure_stage_events(sc);
     Arena ar{sc->base, 0, sc->cap};
@@ -1325,6 +1335,62 @@ int hbls_aggregate_sigs(const uint8_t* sig96, size_t n, uint8_t out96[96]) {
     if (int e = ensure_init()) return e;
     HostLock lk;
     return aggregate_sigs_locked(sig96, n, out96);
+}
+
+// B AggregateSig calls over n signature rows in HBM, shared by the host and device forms: every row decoded once, the sets summed by
+// chunks (kernels.cuh k_g2_segsum_*), the sums serialized into d_out96, the HBLS_AGG_* codes into d_status
+static size_t agg_batch_chunk_cap(size_t B, size_t n) { return (n + HB_AGG_CHUNK - 1) / HB_AGG_CHUNK + B; }
+static size_t agg_batch_scratch_bytes(size_t B, size_t n) {
+    return n * (sizeof(g2a) + 1) + agg_batch_chunk_cap(B, n) * (sizeof(g2) + 1 + 4) + (B + 1) * 8 + B * sizeof(g2) + 8 * 256;
+}
+static void aggregate_sigs_batch_body(size_t B, size_t n, const uint64_t* d_offsets, const uint8_t* d_sigs96, uint8_t* d_out96, uint8_t* d_status,
+                                      cudaStream_t s, Arena& ar) {
+    const size_t cap = agg_batch_chunk_cap(B, n);
+    g2a* pts = ar.take<g2a>(n ? n : 1); uint8_t* ok = ar.take<uint8_t>(n ? n : 1);
+    uint64_t* first = ar.take<uint64_t>(B + 1); uint32_t* chunk_set = ar.take<uint32_t>(cap);
+    g2* part = ar.take<g2>(cap); uint8_t* part_bad = ar.take<uint8_t>(cap); g2* sum = ar.take<g2>(B);
+    if (n) launch_g2_decode_checked(s, n, d_sigs96, pts, ok);
+    LAUNCH(k_g2_segsum_plan, 1, HB_AGG_PLAN_THREADS, s, B, n, d_offsets, cap, first, chunk_set, d_status);
+    LAUNCH(k_g2_segsum_chunks, blocks_for(32 * cap, 128), 128, s, B, (const uint64_t*)d_offsets, (const uint64_t*)first, (const uint32_t*)chunk_set,
+           cap, (const g2a*)pts, (const uint8_t*)ok, part, part_bad);
+    LAUNCH(k_g2_segsum_fold, blocks_for(32 * B, 128), 128, s, B, (const uint64_t*)d_offsets, (const uint64_t*)first, cap, (const g2a*)pts,
+           (const uint8_t*)ok, (const g2*)part, (const uint8_t*)part_bad, sum, d_status);
+    LAUNCH(k_g2_serialize, blocks_for(B, TPB), TPB, s, B, (const g2*)sum, d_out96);
+}
+static int aggregate_sigs_batch_locked(size_t B, const uint64_t* offsets, const uint8_t* sigs96, uint8_t* out96, uint8_t* status) {
+    const size_t n = offsets[B];
+    Scratch* sc; if (int e = reserve(g.stream, agg_batch_scratch_bytes(B, n) + (B + 1) * 8 + n * 96 + B * 97 + 4 * 256, &sc)) return e;
+    Arena ar{sc->base, 0, sc->cap};
+    uint64_t* doff = ar.take<uint64_t>(B + 1); uint8_t* dsig = ar.take<uint8_t>(n ? 96 * n : 1);
+    uint8_t* dout = ar.take<uint8_t>(96 * B); uint8_t* dst = ar.take<uint8_t>(B);
+    CK(cudaMemcpyAsync(doff, offsets, (B + 1) * 8, cudaMemcpyHostToDevice, g.stream));
+    if (n) CK(cudaMemcpyAsync(dsig, sigs96, 96 * n, cudaMemcpyHostToDevice, g.stream));
+    aggregate_sigs_batch_body(B, n, doff, dsig, dout, dst, g.stream, ar);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out96, dout, 96 * B, cudaMemcpyDeviceToHost, g.stream));
+    CK(cudaMemcpyAsync(status, dst, B, cudaMemcpyDeviceToHost, g.stream));
+    CK(cudaStreamSynchronize(g.stream));
+    return 0;
+}
+int hbls_aggregate_sigs_batch(size_t B, const uint64_t* offsets, const uint8_t* sigs96, uint8_t* out96, uint8_t* status) {
+    if (int e = ensure_init()) return e;
+    if (B == 0) return 0;
+    if (!offsets || !out96 || !status || B >= HB_AGG_NO_CHUNK || offsets[0] != 0) return HBLS_ERR_ARG;
+    for (size_t j = 0; j < B; j++) if (offsets[j] > offsets[j + 1]) return HBLS_ERR_ARG;
+    if (offsets[B] > SIZE_MAX / 96 || (offsets[B] && !sigs96)) return HBLS_ERR_ARG;
+    HostLock lk;
+    return aggregate_sigs_batch_locked(B, offsets, sigs96, out96, status);
+}
+int hbls_aggregate_sigs_batch_device(size_t B, size_t n, const void* d_offsets, const void* d_sigs96, void* d_out96, void* d_status, void* stream) {
+    if (int e = ensure_init()) return e;
+    if (B == 0) return 0;
+    if (!d_offsets || ((uintptr_t)d_offsets & 7) || !d_out96 || !d_status || (n && !d_sigs96) || B >= HB_AGG_NO_CHUNK || n > SIZE_MAX / 96)
+        return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    cudaStream_t s = stream ? (cudaStream_t)stream : g.stream;
+    return run_device_form(s, agg_batch_scratch_bytes(B, n), B, [&](Scratch*, Arena& ar) {
+        aggregate_sigs_batch_body(B, n, (const uint64_t*)d_offsets, (const uint8_t*)d_sigs96, (uint8_t*)d_out96, (uint8_t*)d_status, s, ar);
+    }, false);
 }
 
 // ------------------------------------------------------------------ aggregate verification

@@ -225,6 +225,107 @@ __global__ void __launch_bounds__(HB_SUM_THREADS) k_g2_sum(size_t n, const g2a* 
     if (threadIdx.x == 0) out[0] = acc;
 }
 
+// ---- B AggregateSig calls in one launch sequence (hbls_aggregate_sigs_batch): set j = decoded rows offsets[j] .. offsets[j+1]-1.
+// Every set is cut into chunks of at most HB_AGG_CHUNK rows that never cross a set boundary; a warp sums a chunk (k_g2_segsum_chunks),
+// then a warp per set adds its chunk partials (k_g2_segsum_fold).  Summation order is free: only Serialize normalises (A.6).
+#ifndef HB_AGG_CHUNK
+#define HB_AGG_CHUNK 128        // 4 rows per lane: the shuffle tree's 5 Jacobian additions then cost about what the lane's 4 mixed additions
+#endif                          // do, and a 1 000-signature set still spreads over 8 warps (the host emulation shrinks it to a few rows)
+#define HB_AGG_PLAN_THREADS 256
+#define HB_AGG_NO_CHUNK 0xffffffffu                                    // chunk-table slot of a set that is summed by its fold warp
+enum { HB_AGG_OK = 32, HB_AGG_BAD_SIG_ENCODING = 33, HB_AGG_BAD_RANGE = 34 };       // == HBLS_AGG_*
+HB_DEV size_t agg_chunks(size_t len) { return (len + HB_AGG_CHUNK - 1) / HB_AGG_CHUNK; }
+// the 32 lanes' Jacobian sums into lane 0 (5-level shuffle tree); *bad := some lane's flag
+HB_DEV void warp_fold_g2(g2& acc, bool& bad) {
+    const int lane = threadIdx.x & 31;
+    for (int off = 16; off >= 1; off >>= 1) {
+        g2 other; shfl_down_struct(other, acc, off);
+        if (lane < off) pt_add(acc, acc, other);
+    }
+    bad = __ballot_sync(0xffffffffu, bad) != 0;
+}
+// rows b .. e-1 summed by one warp (lane l adds rows b + l, b + l + 32, ...); bad := a row of them did not decode
+HB_DEV void warp_sum_rows(const g2a* __restrict__ pts, const uint8_t* __restrict__ ok, size_t b, size_t e, g2& acc, bool& bad) {
+    pt_set_inf(acc); bad = false;
+    for (size_t i = b + (threadIdx.x & 31); i < e; i += 32) {
+        if (ok[i]) { g2a q = pts[i]; pt_add_mixed(acc, acc, q); }
+        else bad = true;
+    }
+    warp_fold_g2(acc, bad);
+}
+// chunk table (one CTA, any block size): first[j] = exclusive scan of the sets' chunk counts (first[B] = total), chunk_set[c] = the
+// set of chunk c for the chunks below cap; status[j] = HB_AGG_BAD_RANGE for a set whose range is reversed or ends past row n, else 0.
+// Valid sets can overlap when a reversed one lies between them, so the total can exceed cap (the host's bound for disjoint sets,
+// ceil(n / C) + B): a set whose chunks do not all fit marks its slots below cap HB_AGG_NO_CHUNK and is summed by its fold warp.
+__global__ void __launch_bounds__(HB_AGG_PLAN_THREADS) k_g2_segsum_plan(size_t B, size_t n, const uint64_t* __restrict__ offsets, size_t cap,
+                                                                       uint64_t* first, uint32_t* chunk_set, uint8_t* status) {
+    __shared__ uint64_t scan[HB_AGG_PLAN_THREADS];
+    const unsigned t = threadIdx.x, T = blockDim.x;
+    uint64_t carry = 0;
+    for (size_t j0 = 0; j0 < B; j0 += T) {
+        const size_t j = j0 + t;
+        bool good = false; uint64_t cnt = 0;
+        if (j < B) {
+            const uint64_t lo = offsets[j], hi = offsets[j + 1];
+            good = lo <= hi && hi <= n;
+            cnt = good ? agg_chunks(hi - lo) : 0;
+        }
+        scan[t] = cnt;
+        __syncthreads();
+        for (unsigned off = 1; off < T; off <<= 1) {                  // inclusive scan of the tile
+            const uint64_t v = t >= off ? scan[t - off] : 0;
+            __syncthreads();
+            scan[t] += v;
+            __syncthreads();
+        }
+        const uint64_t f = carry + scan[t] - cnt;
+        if (j < B) {
+            first[j] = f; status[j] = good ? 0 : HB_AGG_BAD_RANGE;
+            const uint32_t mark = f + cnt <= cap ? (uint32_t)j : HB_AGG_NO_CHUNK;
+            for (uint64_t c = f; c < f + cnt && c < cap; c++) chunk_set[c] = mark;
+        }
+        carry += scan[T - 1];
+        __syncthreads();                                               // every thread has read the tile total
+    }
+    if (t == 0) first[B] = carry;
+}
+// one warp per chunk-table slot (grid: cap warps; slots at or past the total exit): part[c] = the chunk's sum, part_bad[c] = a row of
+// it did not decode
+__global__ void __launch_bounds__(128, 4) k_g2_segsum_chunks(size_t B, const uint64_t* __restrict__ offsets, const uint64_t* __restrict__ first,
+                                                         const uint32_t* __restrict__ chunk_set, size_t cap, const g2a* __restrict__ pts,
+                                                         const uint8_t* __restrict__ ok, g2* part, uint8_t* part_bad) {
+    const size_t c = HB_TID >> 5;
+    if (c >= cap || c >= first[B]) return;
+    const uint32_t j = chunk_set[c];
+    if (j == HB_AGG_NO_CHUNK) return;
+    const uint64_t b = offsets[j] + (c - first[j]) * HB_AGG_CHUNK, hi = offsets[j + 1];
+    g2* dst = part + c; uint8_t* dst_bad = part_bad + c;
+    g2 acc; bool bad;
+    warp_sum_rows(pts, ok, b, b + HB_AGG_CHUNK < hi ? b + HB_AGG_CHUNK : hi, acc, bad);
+    if ((threadIdx.x & 31) == 0) { *dst = acc; *dst_bad = bad ? 1 : 0; }
+}
+// one warp per set: the sum of its chunk partials (or of its rows, for a set without table slots) into sum[j], the status into status[j];
+// a set with a bad range or an undecodable row gets the identity
+__global__ void __launch_bounds__(128) k_g2_segsum_fold(size_t B, const uint64_t* __restrict__ offsets, const uint64_t* __restrict__ first,
+                                                       size_t cap, const g2a* __restrict__ pts, const uint8_t* __restrict__ ok,
+                                                       const g2* __restrict__ part, const uint8_t* __restrict__ part_bad, g2* sum, uint8_t* status) {
+    const size_t j = HB_TID >> 5;
+    if (j >= B) return;
+    const int lane = threadIdx.x & 31;
+    g2 acc; pt_set_inf(acc); bool bad = false;
+    if (status[j] == HB_AGG_BAD_RANGE) { if (lane == 0) sum[j] = acc; return; }
+    const uint64_t lo = offsets[j], hi = offsets[j + 1], f = first[j], cnt = agg_chunks(hi - lo);
+    if (f + cnt > cap) warp_sum_rows(pts, ok, lo, hi, acc, bad);
+    else {
+        for (uint64_t c = f + lane; c < f + cnt; c += 32) { g2 q = part[c]; pt_add(acc, acc, q); bad |= part_bad[c] != 0; }
+        warp_fold_g2(acc, bad);
+    }
+    if (lane == 0) {
+        if (bad) pt_set_inf(acc);
+        sum[j] = acc; status[j] = bad ? HB_AGG_BAD_SIG_ENCODING : HB_AGG_OK;
+    }
+}
+
 // ---- leader's vote queue into the ballot box (hbls_ballot_box_submit_votes; consensus/leader.go:110-345, quorum.go:164-196,354-377).
 // k_ballot_admit applies the ballot rules in arrival order: vote j's fate depends on the verdicts of the votes before it, so one CTA
 // walks the queue with the box's collected bitmap in shared memory.  Votes are staged into shared memory a chunk at a time (one

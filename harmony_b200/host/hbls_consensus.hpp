@@ -186,6 +186,28 @@ public:
     // order the reference's map iteration sums in (SURVEY A.6)
     bool GetM2Bitmap(uint64_t viewID, Bytes& sig, Bytes& bitmap) { return aggregate(nilSigs, nilBitmap, viewID, sig, bitmap); }
     bool GetM3Bitmap(uint64_t viewID, Bytes& sig, Bytes& bitmap) { return aggregate(viewIDSigs, viewIDBitmap, viewID, sig, bitmap); }
+    // both, as the new leader builds NEWVIEW (view_change_msg.go:119-120), in ONE hbls_aggregate_sigs_batch call: {GetM2Bitmap's,
+    // GetM3Bitmap's} return values and outputs
+    std::pair<bool, bool> GetM2M3Bitmaps(uint64_t viewID, Bytes& m2sig, Bytes& m2bitmap, Bytes& m3sig, Bytes& m3bitmap) {
+        const SigTable* tables[2] = {&nilSigs, &viewIDSigs};
+        const std::map<uint64_t, Bytes>* bitmaps[2] = {&nilBitmap, &viewIDBitmap};
+        Bytes* sig[2] = {&m2sig, &m3sig}; Bytes* bitmap[2] = {&m2bitmap, &m3bitmap};
+        std::vector<std::vector<Bytes>> sets; std::vector<int> which;
+        for (int k = 0; k < 2; k++) {
+            sig[k]->clear(); bitmap[k]->clear();
+            auto it = tables[k]->find(viewID);
+            if (it == tables[k]->end() || it->second.empty()) continue;
+            sets.emplace_back(); for (auto& kv : it->second) sets.back().push_back(kv.second);
+            which.push_back(k);
+        }
+        bool got[2] = {false, false};
+        if (sets.empty()) return {false, false};
+        std::vector<Bytes> aggs;
+        const std::vector<uint8_t> st = bls::AggregateSigBatch(sets, aggs);
+        for (size_t t = 0; t < st.size(); t++)
+            if (st[t] == HBLS_AGG_OK) { const int k = which[t]; *sig[k] = aggs[t]; *bitmap[k] = bitmaps[k]->at(viewID); got[k] = true; }
+        return {got[0], got[1]};
+    }
 
     // a validator receiving NEWVIEW: ParseNewViewMessage's decodes, VerifyNewViewMsg, the M3 quorum and the M1 proof of onNewView:
     // up to three aggregate checks over 8 / 1 / 32-byte messages in ONE hbls_verify_headers call (quorum gate off)

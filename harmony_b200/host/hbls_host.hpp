@@ -160,6 +160,22 @@ inline std::shared_ptr<bls_core::Sign> AggregateSig(const std::vector<bls_core::
     for (auto* s : sigs) agg->Add(s);
     return agg;
 }
+// several AggregateSig calls over serialized signatures in ONE device call (hbls_aggregate_sigs_batch): aggs[j] = the serialized sum
+// of sets[j] (the identity's encoding when one of them does not decode), the return value = the HBLS_AGG_* status per set; empty
+// when the call fails (sizes other than 96 bytes included)
+inline std::vector<uint8_t> AggregateSigBatch(const std::vector<std::vector<std::vector<uint8_t>>>& sets, std::vector<std::vector<uint8_t>>& aggs) {
+    aggs.clear();
+    if (sets.empty()) return {};
+    std::vector<uint64_t> offsets(1, 0); std::vector<uint8_t> blob;
+    for (auto& s : sets) {
+        for (auto& sig : s) { if (sig.size() != 96) return {}; blob.insert(blob.end(), sig.begin(), sig.end()); }
+        offsets.push_back(offsets.back() + s.size());
+    }
+    std::vector<uint8_t> out(96 * sets.size()), status(sets.size());
+    if (hbls_aggregate_sigs_batch(sets.size(), offsets.data(), blob.data(), out.data(), status.data()) != 0) return {};
+    for (size_t j = 0; j < sets.size(); j++) aggs.emplace_back(out.begin() + 96 * j, out.begin() + 96 * (j + 1));
+    return status;
+}
 // bls.go:120-136
 inline bool SeparateSigAndMask(const std::vector<uint8_t>& commitSigs, std::vector<uint8_t>& aggSig, std::vector<uint8_t>& bitmap) {
     if (commitSigs.size() < BLSSignatureSizeInBytes) return false;          // "no mask data found in commit sigs"

@@ -195,6 +195,18 @@ static void test_consensus_messages() {
     Bytes m2s, m2b, m3s, m3b; CHECK(vc.GetM2Bitmap(viewID, m2s, m2b) && vc.GetM3Bitmap(viewID, m3s, m3b) && m2b == Bytes{0x18} && m3b == Bytes{0x1f});
     CHECK(!vc.GetM2Bitmap(viewID + 1, m2s, m2b)); CHECK(vc.GetM2Bitmap(viewID, m2s, m2b));
     { bls_core::Sign manual; for (int i = 0; i < 5; i++) { bls_core::Sign s; CHECK(s.Deserialize(storm[i].ViewidSig)); manual.Add(&s); } CHECK(manual.Serialize() == m3s); }
+    // both aggregates in one batch call, and the batch entry itself on sets with an empty one and an undecodable signature
+    { Bytes s2, b2, s3, b3; const uint64_t l1 = hbls_kernel_launch_count();
+      CHECK(vc.GetM2M3Bitmaps(viewID, s2, b2, s3, b3) == std::make_pair(true, true) && s2 == m2s && b2 == m2b && s3 == m3s && b3 == m3b);
+      const uint64_t one_call = hbls_kernel_launch_count() - l1;
+      CHECK(vc.GetM2M3Bitmaps(viewID + 1, s2, b2, s3, b3) == std::make_pair(false, false) && s2.empty() && b3.empty());
+      CHECK(hbls_kernel_launch_count() - l1 == one_call);                            // nobody signed: no device call
+      std::vector<Bytes> aggs;
+      const auto st = bls::AggregateSigBatch({{storm[0].ViewidSig, storm[1].ViewidSig}, {}, {storm[0].ViewidSig, Bytes(96, 0xff)}}, aggs);
+      bls_core::Sign ident; const Bytes id96 = ident.Serialize();
+      CHECK(st == (std::vector<uint8_t>{HBLS_AGG_OK, HBLS_AGG_OK, HBLS_AGG_BAD_SIG_ENCODING}) && aggs.size() == 3 && aggs[1] == id96 && aggs[2] == id96);
+      bls_core::Sign two; for (int i = 0; i < 2; i++) { bls_core::Sign s; CHECK(s.Deserialize(storm[i].ViewidSig)); two.Add(&s); }
+      CHECK(aggs[0] == two.Serialize()); }
     FBFTMessage nv; nv.ViewID = viewID; nv.BlockNum = 9; nv.SenderPubkey = storm[0].SenderPubkey; nv.Payload = payload; nv.Block = {0xc0};
     nv.hasM2 = nv.hasM3 = true; nv.M2AggSig = m2s; nv.M2Bitmap = m2b; nv.M3AggSig = m3s; nv.M3Bitmap = m3b;
     viewChange validator; CHECK(validator.Init(pubs).empty());

@@ -119,6 +119,28 @@ int hbls_mask_aggregate(const hbls_committee* c, const uint8_t* bitmap, size_t b
  * decode n signatures (with subgroup check) and sum them.  0 ok, HBLS_ERR_DECODE if one fails. */
 int hbls_aggregate_sigs(const uint8_t* sig96, size_t n, uint8_t out96[96]);
 
+/* B independent AggregateSig calls (crypto/bls/mask.go:58-64; quorum.go:164-196; view_change_msg.go:119-120: the new leader's M2 and
+ * M3 aggregates; a sweep of rounds of one committee).
+ * Set j = signatures offsets[j] .. offsets[j+1]-1 of sigs96 (96 B each); offsets: B+1 values, offsets[0] = 0, non-decreasing.
+ * out96 + 96 j = Serialize(sum of set j) -- byte for byte what hbls_aggregate_sigs writes for that set when it returns 0;
+ * an empty set gives the identity's encoding.  status[j]:
+ *   HBLS_AGG_OK                 every signature of the set decoded (subgroup check included)
+ *   HBLS_AGG_BAD_SIG_ENCODING   some signature of the set does not decode; out96 + 96 j = the identity's encoding
+ *   HBLS_AGG_BAD_RANGE          (device form only) offsets[j] > offsets[j+1] or offsets[j+1] > n; out = the identity's encoding
+ * The codes are distinct from HBLS_VB_*, HBLS_HDR_* and HBLS_BALLOT_*, so a status array cannot be read under the wrong table.
+ * Every signature is decoded once; a set is summed by chunks of at most 128 signatures on many SMs at once.
+ * 0 ok (B == 0: nothing launched), HBLS_ERR_ARG (null pointers with B > 0, bad host offsets), HBLS_ERR_CUDA.  The host form takes
+ * the library lock like the other batch entries; it is not combined with other calls and does not set hbls_last_batch_info. */
+#define HBLS_AGG_OK               32
+#define HBLS_AGG_BAD_SIG_ENCODING 33
+#define HBLS_AGG_BAD_RANGE        34
+int hbls_aggregate_sigs_batch(size_t B, const uint64_t* offsets, const uint8_t* sigs96, uint8_t* out96, uint8_t* status);
+/* device form (rules of the device forms below, capture included): every d_ pointer in HBM, d_offsets 8-byte aligned (B+1 uint64
+ * values, not checked on the host: a bad range gives HBLS_AGG_BAD_RANGE); n = number of signature rows at d_sigs96 (host-known,
+ * sizes scratch and grids).  It draws no coefficients: hbls_get_param("rlc_draws") does not move, captured or not. */
+int hbls_aggregate_sigs_batch_device(size_t B, size_t n, const void* d_offsets, const void* d_sigs96,
+                                     void* d_out96, void* d_status, void* stream);
+
 /* FastAggregateVerify / VerifyAggregateSig of BASELINE.json == the reference composition
  * Deserialize(sig) ; SetMask(bitmap) ; aggSig.VerifyHash(mask.AggregatePublic, msg)
  * (internal/chain/engine.go:630-640, consensus/validator.go:219-236).  1 valid, 0 invalid, <0 error.  HBLS_ERR_ARG for a null
@@ -228,7 +250,8 @@ int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96
  * message is hashed to G2 once.  The H(m) cache is neither read nor filled (hbls_hash_cache_stats does not move).
  * The first call on a stream, or one larger than any before it there, allocates scratch (which may wait for the device); the items
  * form also waits, on the host, for the upload of the previous items call on the same stream if that has not run yet.
- * CUDA graphs: hbls_verify_batch_status_device, hbls_verify_headers_device and hbls_aggregate_verify_batch_device may be called on a
+ * CUDA graphs: hbls_verify_batch_status_device, hbls_verify_headers_device, hbls_aggregate_verify_batch_device and
+ * hbls_aggregate_sigs_batch_device (which draws nothing and sets no batch info) may be called on a
  * stream that is capturing (cudaStreamBeginCapture, torch.cuda.graph), with no warm-up call.  The call then becomes part of the
  * caller's graph: its scratch comes from cudaMallocAsync / cudaFreeAsync on that stream, so every replay gets scratch of its own
  * (shared with no direct call and no other graph, released with the graph), and the random-linear-combination coefficients and the
