@@ -118,13 +118,14 @@ int ensure_init() {
     return HBLS_ERR_CUDA;
 }
 
+// Byte layout of a call's buffers: 256-byte aligned takes, a zero-length take gets one element.  Over base 0 it only measures: a carve
+// function run on Arena{} gives the bytes it needs (off), run again over real memory the same takes hand out the buffers.  offset<T>
+// gives the same layout for packed host staging copies.
 struct Arena {
-    uint8_t* base; size_t off = 0, cap;
-    template <class T> T* take(size_t n) {
-        off = (off + 255) & ~(size_t)255;
-        T* p = reinterpret_cast<T*>(base + off); off += n * sizeof(T);
-        return p;
-    }
+    uintptr_t base = 0; size_t off = 0;
+    template <class T> size_t offset(size_t n) { const size_t at = (off + 255) & ~(size_t)255; off = at + (n ? n : 1) * sizeof(T); return at; }
+    template <class T> T* take(size_t n) { return reinterpret_cast<T*>(base + offset<T>(n)); }
+    template <class F> static size_t bytes(F carve) { Arena a; carve(a); return a.off; }
 };
 // scratch of stream s, grown to `bytes` (growing frees the old block: cudaFree waits for the device, so no kernel still reads it)
 int reserve(cudaStream_t s, size_t bytes, Scratch** out) {
@@ -147,6 +148,14 @@ int reserve(cudaStream_t s, size_t bytes, Scratch** out) {
     sc.forked = false; sc.ev7_set = false;
     *out = &sc;
     return 0;
+}
+// the buffers of one call on stream s: carve(ar) takes all of them and returns them.  Measured first, then carved from the stream's
+// scratch grown to that size (*sc_out, when given).  *err: 0, or reserve's error (the buffers returned are then not to be used).
+template <class F> auto carve_scratch(cudaStream_t s, int* err, F carve, Scratch** sc_out = nullptr) {
+    Scratch* sc = nullptr; *err = reserve(s, Arena::bytes(carve), &sc);
+    if (sc_out) *sc_out = sc;
+    Arena ar{*err ? 0 : (uintptr_t)sc->base};
+    return carve(ar);
 }
 inline unsigned blocks_for(size_t n, unsigned tpb) { return (unsigned)((n + tpb - 1) / tpb); }
 
@@ -293,15 +302,11 @@ size_t rlc_lines_bytes(size_t B) {
 }
 // blocks per call at most: S <= ceil(ng / HB_RLC_M) + 31
 size_t rlc_nblocks_max(size_t B) { return B / HB_RLC_G / HB_RLC_M + 32; }
-size_t verify_scratch_bytes(size_t B) {
-    return B * (sizeof(g2a) * 2 + sizeof(g1a) * 2 + sizeof(g1) + sizeof(g2) + 16 + 4 + 7) + HB_MASK_BINS * 4 + (B / HB_RLC_G + 1) * (sizeof(g2a) + 8) + rlc_nblocks_max(B) * (sizeof(g2a) + 1) + 46 * 256
-           + (B <= 8192 ? B * (12 * sizeof(fp2) + 3) + 1024 : 0)                // latency path: Miller values of (B, sigma) and (-apk, H(m))
-           + rlc_lines_bytes(B);                                                 // two-kernel pairing: the line functions of one chunk
-}
+// flags: the packed decode flags of the status forms (k_pack_flags)
 struct VerifyBufs { g2a* sig; g2a* hm; g1a* pkneg; g1* apk; uint8_t* ok_sig; uint8_t* ok_hm; uint8_t* ok_pk;
                     g1a* pk_scaled; g2* S; uint8_t* bad; g2a* Sg; uint8_t* group_ok; uint32_t* fail_list; unsigned* counts; g2a* Sb; uint8_t* block_ok;
                     fp2* f1; uint8_t* irr1; fp2* f2; uint8_t* irr2; uint8_t* ok_sub;
-                    uint16_t* mask_cost; unsigned* mask_hist; uint32_t* mask_order; fp* lines; uint8_t* verdict; };
+                    uint16_t* mask_cost; unsigned* mask_hist; uint32_t* mask_order; fp* lines; uint8_t* verdict; uint8_t* flags; };
 VerifyBufs carve_verify(Arena& ar, size_t B) {
     VerifyBufs v;
     v.sig = ar.take<g2a>(B); v.hm = ar.take<g2a>(B); v.pkneg = ar.take<g1a>(B); v.apk = ar.take<g1>(B);
@@ -311,7 +316,7 @@ VerifyBufs carve_verify(Arena& ar, size_t B) {
     v.fail_list = ar.take<uint32_t>(B); v.counts = ar.take<unsigned>(5);      // [0] [1] k_rlc_finish, [2] [3] form gates, [4] per-group check list
     v.Sb = ar.take<g2a>(rlc_nblocks_max(B)); v.block_ok = ar.take<uint8_t>(rlc_nblocks_max(B));
     v.mask_cost = ar.take<uint16_t>(B); v.mask_hist = ar.take<unsigned>(HB_MASK_BINS); v.mask_order = ar.take<uint32_t>(B);
-    v.verdict = ar.take<uint8_t>(B);
+    v.verdict = ar.take<uint8_t>(B); v.flags = ar.take<uint8_t>(B);
     v.lines = nullptr;
     if (rlc_lines_bytes(B)) v.lines = reinterpret_cast<fp*>(ar.take<uint8_t>(rlc_lines_bytes(B)));
     v.f1 = v.f2 = nullptr; v.irr1 = v.irr2 = v.ok_sub = nullptr;
@@ -347,7 +352,6 @@ void launch_exact_two_phase(size_t n, const g2a* sig, const g1a* pkneg, const g2
 struct MsgGroups { uint32_t mask; uint32_t* slot_item; uint32_t* slot_rep; uint32_t* item_slot; uint32_t* pos; uint32_t* grp; uint8_t* keys;
                    unsigned* count; g2a* hm_d; uint8_t* ok_d; };
 size_t group_slots(size_t k) { size_t T = 64; while (T < 2 * k) T <<= 1; return T; }
-size_t group_bytes(size_t k) { return group_slots(k) * 8 + k * (12 + 48 + sizeof(g2a) + 1) + 10 * 256; }
 MsgGroups carve_groups(Arena& ar, size_t k) {
     MsgGroups m; const size_t T = group_slots(k);
     m.mask = (uint32_t)(T - 1); m.slot_item = ar.take<uint32_t>(T); m.slot_rep = ar.take<uint32_t>(T);
@@ -642,11 +646,43 @@ struct Part1Req : hbls_coalesce::Request {
 };
 static bool is_verify(int kind) { return kind == RQ_VERIFY || kind == RQ_AGG || kind == RQ_MASK; }
 static_assert(sizeof(g1) == sizeof(blsPublicKey) && sizeof(g2) == sizeof(blsSignature), "herumi struct layout");
-// byte layout of one staging copy: 256-byte aligned sections
-struct Layout {
-    size_t size = 0;
-    size_t put(size_t bytes) { const size_t off = (size + 255) & ~(size_t)255; size = off + (bytes ? bytes : 1); return off; }
+
+// The H(m) table of a call that hashes on the host's request (part1_locked, sign_hash_keys_locked): one entry per distinct message
+// (the key hm_key builds), the misses at the front (contiguous: one hash launch), the entries the cache holds at the back.
+// keys[d] = the distinct keys in order of first appearance, pos[d] = the table entry of keys[d], entry[i] = the table entry of message i
+struct HmTable {
+    std::vector<std::array<uint8_t, 48>> keys; std::vector<uint32_t> pos, entry; std::vector<bool> cached; size_t nmiss = 0;
+    // the miss keys, 48 bytes at each miss's entry: the host staging of hm_table_fill's d_keys
+    void stage_misses(uint8_t* dst) const { for (size_t d = 0; d < keys.size(); d++) if (!cached[d]) memcpy(dst + 48 * pos[d], keys[d].data(), 48); }
 };
+// msg(i) = {bytes, length} of message i < n
+template <class F> HmTable hm_table(size_t n, F msg) {
+    HmTable t; t.entry.resize(n);
+    std::map<std::array<uint8_t, 48>, uint32_t> seen;
+    for (size_t i = 0; i < n; i++) {
+        const auto [p, len] = msg(i);
+        std::array<uint8_t, 48> k; hm_key(k.data(), p, len);
+        auto it = seen.emplace(k, (uint32_t)t.keys.size());
+        if (it.second) t.keys.push_back(k);
+        t.entry[i] = it.first->second;
+    }
+    const size_t nk = t.keys.size();
+    t.pos.resize(nk); t.cached.assign(nk, false);
+    for (size_t d = 0; d < nk; d++) t.cached[d] = hm_enabled() && hm_find(t.keys[d].data()) >= 0;
+    for (size_t d = 0, hit = 0; d < nk; d++) t.pos[d] = t.cached[d] ? (uint32_t)(nk - 1 - hit++) : (uint32_t)t.nmiss++;
+    for (uint32_t& e : t.entry) e = t.pos[e];
+    return t;
+}
+// the table's points into th / tok on stream s: cached entries (this node signed, verified or prefetched the message before), then one
+// launch over the misses staged at d_keys, which the cache keeps
+void hm_table_fill(const HmTable& t, const uint8_t* d_keys, g2a* th, uint8_t* tok, cudaStream_t s) {
+    for (size_t d = 0; d < t.keys.size(); d++) if (t.cached[d]) hm_fetch(t.keys[d].data(), th + t.pos[d], tok + t.pos[d], s);
+    if (hm_enabled()) g.hm_misses += t.nmiss;
+    if (t.nmiss) {
+        launch_hash_small(s, t.nmiss, d_keys, 48, th, tok);
+        if (hm_enabled()) for (size_t d = 0; d < t.keys.size(); d++) if (!t.cached[d]) hm_store(t.keys[d].data(), th + t.pos[d], tok + t.pos[d], s);
+    }
+}
 
 // One turn: the requests rq[0..n) under g.mu.  d_apk / sig96 (a lone hbls_mask_verify: one verify request): the key is already on
 // the device and the signature is serialized (decoded and subgroup-checked here).  Otherwise the verify requests run in the order
@@ -680,44 +716,33 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
         std::copy(rest.begin(), rest.end(), sgn.begin() + ngls);
     }
     const size_t nv = ver.size(), ns = sgn.size(), np = pub.size(), n1 = one.size(), nh = nv + ns;
-    // H(m): one table entry per distinct message of the verify and sign requests (the key hm_key builds); entries the cache holds at
-    // the back, the misses at the front (contiguous: one hash launch), idx[i] = entry of request i (verify requests, then sign)
-    std::vector<std::array<uint8_t, 48>> keys; std::vector<uint32_t> idx(nh);
-    {
-        std::map<std::array<uint8_t, 48>, uint32_t> seen;
-        for (size_t i = 0; i < nh; i++) {
-            const Part1Req* r = i < nv ? ver[i] : sgn[i - nv];
-            std::array<uint8_t, 48> k; hm_key(k.data(), r->msg, r->len);
-            auto it = seen.emplace(k, (uint32_t)keys.size());
-            if (it.second) keys.push_back(k);
-            idx[i] = it.first->second;
-        }
-    }
-    const size_t nk = keys.size();
-    std::vector<uint32_t> pos(nk); std::vector<bool> cached(nk, false); size_t nmiss = 0;
-    for (size_t d = 0; d < nk; d++) cached[d] = hm_enabled() && hm_find(keys[d].data()) >= 0;
-    for (size_t d = 0, hit = 0; d < nk; d++) pos[d] = cached[d] ? (uint32_t)(nk - 1 - hit++) : (uint32_t)nmiss++;
+    // H(m) of the verify requests, then the sign requests: hm_tab.entry[i] = table entry of request i
+    const HmTable hm_tab = hm_table(nh, [&](size_t i) { const Part1Req* r = i < nv ? ver[i] : sgn[i - nv]; return std::pair{r->msg, r->len}; });
+    const size_t nk = hm_tab.keys.size();
     bool gather = nk != nh;
-    for (size_t i = 0; i < nh; i++) { idx[i] = pos[idx[i]]; gather |= idx[i] != i; }
+    for (size_t i = 0; i < nh; i++) gather |= hm_tab.entry[i] != i;
     // staging (host -> device, one copy) and results (device -> host, one copy)
-    Layout in, out;
-    const size_t i_apk = d_apk ? 0 : in.put(nv * sizeof(g1)), i_sig = in.put(sig96 ? 96 : (nv - nser) * sizeof(g2)), i_keys = in.put(nmiss * 48);
+    Arena in, out;
+    const size_t i_apk = d_apk ? 0 : in.offset<g1>(nv), i_sig = in.offset<uint8_t>(sig96 ? 96 : (nv - nser) * sizeof(g2)), i_keys = in.offset<uint8_t>(hm_tab.nmiss * 48);
     // AGG / MASK: the serialized signatures, the decode flags of every verify request, the mask_item descriptors and their bitmaps
-    const size_t i_ser = nser ? in.put(nser * 96) : 0, i_sok = nser ? in.put(nv) : 0;
-    const size_t i_items = na ? in.put(na * sizeof(mask_item)) : 0, i_bm = na ? in.put(bm_bytes) : 0;
-    const size_t i_idx = gather ? in.put(nh * 4) : 0, i_dig = in.put(dig.size() * 8), i_sk = in.put((ns - ngls) * 32), i_pub = in.put(np * 32);
+    const size_t i_ser = nser ? in.offset<uint8_t>(nser * 96) : 0, i_sok = nser ? in.offset<uint8_t>(nv) : 0;
+    const size_t i_items = na ? in.offset<mask_item>(na) : 0, i_bm = na ? in.offset<uint8_t>(bm_bytes) : 0;
+    const size_t i_idx = gather ? in.offset<uint32_t>(nh) : 0, i_dig = in.offset<uint64_t>(dig.size()), i_sk = in.offset<uint8_t>((ns - ngls) * 32);
+    const size_t i_pub = in.offset<uint8_t>(np * 32);
     std::vector<size_t> i_a(n1), i_b(n1), o_out(n1);
-    for (size_t j = 0; j < n1; j++) { i_a[j] = in.put(one[j]->an); i_b[j] = in.put(one[j]->bn); o_out[j] = out.put(one[j]->on); }
-    const size_t i_desc = n1 > 1 ? in.put(n1 * sizeof(single_desc)) : 0;
-    const size_t o_res = out.put(nv), o_sig = out.put(ns * sizeof(g2)), o_sok = out.put(ns), o_pub = out.put(np * sizeof(g1)), o_rc = out.put(n1 * sizeof(int));
-    Scratch* sc;
-    if (int e = reserve(s, in.size + out.size + nv * (sizeof(g1a) + sizeof(g2a) + 1) + (nk + nh) * (sizeof(g2a) + 1) + 16 * 256, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* din = ar.take<uint8_t>(in.size); uint8_t* dout = ar.take<uint8_t>(out.size);
-    g1a* pkneg = ar.take<g1a>(nv); g2a* vsig = ar.take<g2a>(nv); uint8_t* ok_sig = ar.take<uint8_t>(nv);
-    g2a* hm = ar.take<g2a>(nh); uint8_t* ok_hm = ar.take<uint8_t>(nh);
-    g2a* th = gather ? ar.take<g2a>(nk) : hm; uint8_t* tok = gather ? ar.take<uint8_t>(nk) : ok_hm;      // the H(m) table
-    std::vector<uint8_t> hin(in.size), hout(out.size);
+    for (size_t j = 0; j < n1; j++) { i_a[j] = in.offset<uint8_t>(one[j]->an); i_b[j] = in.offset<uint8_t>(one[j]->bn); o_out[j] = out.offset<uint8_t>(one[j]->on); }
+    const size_t i_desc = n1 > 1 ? in.offset<single_desc>(n1) : 0;
+    const size_t o_res = out.offset<uint8_t>(nv), o_sig = out.offset<g2>(ns), o_sok = out.offset<uint8_t>(ns), o_pub = out.offset<g1>(np);
+    const size_t o_rc = out.offset<int>(n1);
+    Scratch* sc; int err; const auto [din, dout, pkneg, vsig, ok_sig, hm, ok_hm, th, tok] = carve_scratch(s, &err, [&](Arena& ar) {
+        uint8_t* din = ar.take<uint8_t>(in.off); uint8_t* dout = ar.take<uint8_t>(out.off);
+        g1a* pkneg = ar.take<g1a>(nv); g2a* vsig = ar.take<g2a>(nv); uint8_t* ok_sig = ar.take<uint8_t>(nv);
+        g2a* hm = ar.take<g2a>(nh); uint8_t* ok_hm = ar.take<uint8_t>(nh);
+        g2a* th = gather ? ar.take<g2a>(nk) : hm; uint8_t* tok = gather ? ar.take<uint8_t>(nk) : ok_hm;      // the H(m) table
+        return std::tuple{din, dout, pkneg, vsig, ok_sig, hm, ok_hm, th, tok};
+    }, &sc);
+    if (err) return err;
+    std::vector<uint8_t> hin(in.off), hout(out.off);
     // the digit, key and GetPublicKey sections are adjacent: [key_lo, key_hi) holds every secret byte of the staging copy.  The host copy
     // is wiped on every return path, the device copy on the stream after the ladder kernels.
     const size_t key_lo = i_dig, key_hi = i_pub + np * 32;
@@ -736,8 +761,8 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
             off += r.blen;
         }
     }
-    for (size_t d = 0; d < nk; d++) if (!cached[d]) memcpy(&hin[i_keys + 48 * pos[d]], keys[d].data(), 48);
-    if (gather) memcpy(&hin[i_idx], idx.data(), nh * 4);
+    hm_tab.stage_misses(&hin[i_keys]);
+    if (gather) memcpy(&hin[i_idx], hm_tab.entry.data(), nh * 4);
     if (!dig.empty()) memcpy(&hin[i_dig], dig.data(), dig.size() * 8);
     for (size_t i = ngls; i < ns; i++) memcpy(&hin[i_sk + 32 * (i - ngls)], static_cast<const blsSecretKey*>(sgn[i]->a)->d, 32);
     for (size_t i = 0; i < np; i++) memcpy(&hin[i_pub + 32 * i], static_cast<const blsSecretKey*>(pub[i]->a)->d, 32);
@@ -748,7 +773,7 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
         desc[j] = single_desc{din + i_a[j], din + i_b[j], dout + o_out[j], one[j]->op, (uint32_t)one[j]->len};
     }
     if (n1 > 1) memcpy(&hin[i_desc], desc.data(), n1 * sizeof(single_desc));
-    CK(cudaMemcpyAsync(din, hin.data(), in.size, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(din, hin.data(), in.off, cudaMemcpyHostToDevice, s));
     int* drc = reinterpret_cast<int*>(dout + o_rc);
     if (n1) LAUNCH(k_single, blocks_for(n1, 32), 32, s, n1, n1 > 1 ? (const single_desc*)(din + i_desc) : (const single_desc*)nullptr, desc[0], drc);
     if (np) LAUNCH(k_g1_mul_gen, blocks_for(np, 32), 32, s, np, (const uint8_t*)(din + i_pub), reinterpret_cast<g1*>(dout + o_pub));
@@ -764,13 +789,7 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
             if (nv > nser) LAUNCH(k_g2_normalize, blocks_for(nv - nser, 32), 32, s, nv - nser, reinterpret_cast<const g2*>(din + i_sig), vsig + nser);
         }
     }
-    // H(m): cached entries (this node signed, verified or prefetched the message before), then one launch over the misses
-    for (size_t d = 0; d < nk; d++) if (cached[d]) hm_fetch(keys[d].data(), th + pos[d], tok + pos[d], s);
-    if (hm_enabled()) g.hm_misses += nmiss;
-    if (nmiss) {
-        launch_hash_small(s, nmiss, din + i_keys, 48, th, tok);
-        if (hm_enabled()) for (size_t d = 0; d < nk; d++) if (!cached[d]) hm_store(keys[d].data(), th + pos[d], tok + pos[d], s);
-    }
+    hm_table_fill(hm_tab, din + i_keys, th, tok, s);
     if (gather) LAUNCH(k_broadcast_hm, blocks_for(nh, 256), 256, s, nh, (const uint32_t*)(din + i_idx), (const g2a*)th, (const uint8_t*)tok, hm, ok_hm);
     if (nv) {
         uint8_t* dres = dout + o_res;
@@ -785,7 +804,7 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
                           (size_t)1, dsig_out + ngls, dsok + ngls);
     if (ns || np) CK(cudaMemsetAsync(din + key_lo, 0, key_hi - key_lo, s));
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(hout.data(), dout, out.size, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(hout.data(), dout, out.off, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     if (na) {            // committee checks in the turn: an exact-mode batch of na rounds, a warp per round (hbls_last_batch_info)
         g.info = hbls_batch_info{}; g.info.mode = 0; g.info.rounds = na; g.info.cta_threads = 32;
@@ -944,11 +963,10 @@ void launch_mask_serial(const hbls_committee* c, size_t B, const uint8_t* d_bitm
     }
     LAUNCH(k_mask_aggregate_serial, light_blocks(B), TPB, s, B, c->n, c->table, c->total, d_bitmaps, blen, v.apk, order);
 }
-// rounds against one committee, everything device-resident
-int agg_verify_device_locked(const hbls_committee* c, size_t B, const uint8_t* d_bitmaps, size_t blen, const uint8_t* d_sigs,
-                             const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, Arena& ar, bool same_msg,
-                             VerifyBufs* v_out = nullptr, const uint8_t* h_msg = nullptr, const MsgGroups* mg = nullptr) {
-    VerifyBufs v = carve_verify(ar, B);
+// rounds against one committee, everything device-resident; v = carve_verify(B)
+void agg_verify_device_locked(const hbls_committee* c, size_t B, const uint8_t* d_bitmaps, size_t blen, const uint8_t* d_sigs,
+                              const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, const VerifyBufs& v,
+                              bool same_msg, const uint8_t* h_msg = nullptr, const MsgGroups* mg = nullptr) {
     fork_point(B, sc, s);
     STAGE_EV(0, sc, s);
     if (B >= (size_t)g.sm_count * 256)
@@ -956,8 +974,6 @@ int agg_verify_device_locked(const hbls_committee* c, size_t B, const uint8_t* d
     else
         LAUNCH(k_mask_aggregate, blocks_for(B * 32, 128), 128, s, B, c->n, c->table, d_bitmaps, blen, v.apk);
     launch_verify_tail(B, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, same_msg, h_msg, mg);
-    if (v_out) *v_out = v;
-    return 0;
 }
 // Mask.SetMask with g.mu held (bitmap: m->bitmap.size() bytes)
 int set_mask_locked(hbls_mask* m, const uint8_t* bitmap) {
@@ -970,9 +986,8 @@ int set_mask_locked(hbls_mask* m, const uint8_t* bitmap) {
         if (was && !now) { delta[blen + (i >> 3)] |= msk; any = true; }
     }
     if (!any) return 0;
-    Scratch* sc; if (int e = reserve(g.stream, 2 * blen + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dbm = ar.take<uint8_t>(2 * blen + 2); g1* dtmp = ar.take<g1>(2); int* drc = ar.take<int>(1);
+    int err; const auto [dbm, dtmp, drc] = carve_scratch(g.stream, &err, [&](Arena& ar) { return std::tuple{ar.take<uint8_t>(2 * blen + 2), ar.take<g1>(2), ar.take<int>(1)}; });
+    if (err) return err;
     CK(cudaMemcpyAsync(dbm, delta.data(), 2 * blen, cudaMemcpyHostToDevice, g.stream));
     LAUNCH(k_mask_aggregate, 1, 64, g.stream, (size_t)2, n, m->c->table, dbm, blen, dtmp);
     LAUNCH(k_single, 1, 32, g.stream, (size_t)1, (const single_desc*)nullptr, single_desc{m->d_acc, dtmp + 0, m->d_acc, OP_G1_ADD, 0u}, drc);
@@ -998,37 +1013,34 @@ int capturing(cudaStream_t s) {
     CK(cudaStreamIsCapturing(s, &cs));
     return cs != cudaStreamCaptureStatusNone ? 1 : 0;
 }
-// body(sc, ar) enqueues the call's B rounds / items on s with the arena ar of `bytes`; sc is a stand-in that is never used while
-// g.cap_draw is set (no fork, no stage events, no counters).  draw = false: the call uses no coefficients (g.cap_draw stays null,
-// rlc_draws does not move), and its body touches no Scratch state either.
-template <class F> int run_captured(cudaStream_t s, size_t bytes, size_t B, F body, bool draw = true) {
-    bytes += sizeof(rlc_draw_out) + 256;
+// body(sc, bufs) enqueues the call's B rounds / items on s with the buffers bufs = carve(ar) takes; sc is a stand-in that is never
+// used while g.cap_draw is set (no fork, no stage events, no counters).  draw = false: the call uses no coefficients (g.cap_draw stays
+// null, rlc_draws does not move), and its body touches no Scratch state either.
+template <class C, class F> int run_captured(cudaStream_t s, size_t B, C carve, F body, bool draw) {
+    auto layout = [&](Arena& ar) { rlc_draw_out* drawn = draw ? ar.take<rlc_draw_out>(1) : nullptr; return std::pair{drawn, carve(ar)}; };
     uint8_t* base = nullptr;
-    CK(cudaMallocAsync(reinterpret_cast<void**>(&base), bytes, s));
-    Arena ar{base, 0, bytes};
-    rlc_draw_out* drawn = nullptr;
-    if (draw) {
-        drawn = ar.take<rlc_draw_out>(1);
-        LAUNCH(k_rlc_draw, 1, 32, s, (const uint32_t*)g.d_chacha_key, g.d_draws, HB_RLC_DRAW_NONCE, rlc_applies(B) ? 18u : 2u, drawn);
-    }
+    CK(cudaMallocAsync(reinterpret_cast<void**>(&base), Arena::bytes(layout), s));
+    Arena ar{(uintptr_t)base};
+    const auto [drawn, bufs] = layout(ar);
+    if (draw) LAUNCH(k_rlc_draw, 1, 32, s, (const uint32_t*)g.d_chacha_key, g.d_draws, HB_RLC_DRAW_NONCE, rlc_applies(B) ? 18u : 2u, drawn);
     Scratch stand_in;
     g.cap_draw = drawn;
-    body(&stand_in, ar);
+    body(&stand_in, bufs);
     g.cap_draw = nullptr;
     const cudaError_t launched = cudaGetLastError();
     CK(cudaFreeAsync(base, s));
     if (launched != cudaSuccess) { note_error(launched, "launch", __FILE__, __LINE__); return HBLS_ERR_CUDA; }
     return 0;
 }
-// a device form's call: captured, or in the stream's arena (reserve) as it always was
-template <class F> int run_device_form(cudaStream_t s, size_t bytes, size_t B, F body, bool draw = true) {
+// a device form's call: captured, or in the stream's scratch as it always was
+template <class C, class F> int run_device_form(cudaStream_t s, size_t B, C carve, F body, bool draw = true) {
     const int cap = capturing(s);
     if (cap < 0) return cap;
-    if (cap) return run_captured(s, bytes, B, body, draw);
-    Scratch* sc; if (int e = reserve(s, bytes, &sc)) return e;
+    if (cap) return run_captured(s, B, carve, body, draw);
+    Scratch* sc; int err; const auto bufs = carve_scratch(s, &err, carve, &sc);
+    if (err) return err;
     ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    body(sc, ar);
+    body(sc, bufs);
     CK(cudaGetLastError());
     return 0;
 }
@@ -1207,9 +1219,8 @@ int hbls_hash_prefetch(const void* msg, size_t msg_len) {
     uint8_t key[48]; hm_key(key, msg, msg_len);
     if (const int i = hm_find(key); i >= 0) { g.hm[i].stamp = ++g.hm_clock; return 0; }
     cudaStream_t st = g.aux[1];
-    Scratch* sc; if (int e = reserve(st, 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dmsg = ar.take<uint8_t>(64); g2a* dhm = ar.take<g2a>(1); uint8_t* dok = ar.take<uint8_t>(1);
+    int err; const auto [dmsg, dhm, dok] = carve_scratch(st, &err, [](Arena& ar) { return std::tuple{ar.take<uint8_t>(64), ar.take<g2a>(1), ar.take<uint8_t>(1)}; });
+    if (err) return err;
     // the 48 key bytes ARE the bytes hash_to_fp reads (pageable source: the runtime stages it before cudaMemcpyAsync returns)
     CK(cudaMemcpyAsync(dmsg, key, 48, cudaMemcpyHostToDevice, st));
     launch_hash_small(st, 1, dmsg, 48, dhm, dok);
@@ -1270,9 +1281,8 @@ static int committee_create_locked(hbls_committee** out, const uint8_t* pk48, si
     std::unique_ptr<hbls_committee> c(new hbls_committee); c->n = n;       // freed (with its device tables) on every early return
     size_t nn = n ? n : 1;
     CK(cudaMalloc(&c->table, nn * sizeof(g1a)));
-    Scratch* sc; if (int e = reserve(g.stream, nn * 49 + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* din = ar.take<uint8_t>(nn * 48); uint8_t* dok = ar.take<uint8_t>(nn);
+    int err; const auto [din, dok] = carve_scratch(g.stream, &err, [&](Arena& ar) { return std::tuple{ar.take<uint8_t>(nn * 48), ar.take<uint8_t>(nn)}; });
+    if (err) return err;
     std::vector<uint8_t> ok(nn, 1);
     if (n) {
         CK(cudaMemcpyAsync(din, pk48, n * 48, cudaMemcpyHostToDevice, g.stream));
@@ -1295,9 +1305,8 @@ void hbls_committee_destroy(hbls_committee* c) { if (!c) return; HostLock lk; cu
 size_t hbls_committee_size(const hbls_committee* c) { return c ? c->n : 0; }
 
 static int mask_aggregate_locked(const hbls_committee* c, const uint8_t* bitmap, size_t blen, uint8_t out_pk48[48]) {
-    Scratch* sc; if (int e = reserve(g.stream, blen + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dbm = ar.take<uint8_t>(blen ? blen : 1); g1* dacc = ar.take<g1>(1); uint8_t* dout = ar.take<uint8_t>(48);
+    int err; const auto [dbm, dacc, dout] = carve_scratch(g.stream, &err, [&](Arena& ar) { return std::tuple{ar.take<uint8_t>(blen), ar.take<g1>(1), ar.take<uint8_t>(48)}; });
+    if (err) return err;
     if (blen) CK(cudaMemcpyAsync(dbm, bitmap, blen, cudaMemcpyHostToDevice, g.stream));
     LAUNCH(k_mask_aggregate, 1, 32, g.stream, (size_t)1, c->n, c->table, dbm, blen, dacc);
     LAUNCH(k_g1_serialize, 1, 32, g.stream, (size_t)1, dacc, dout);
@@ -1314,10 +1323,10 @@ int hbls_mask_aggregate(const hbls_committee* c, const uint8_t* bitmap, size_t b
 
 static int aggregate_sigs_locked(const uint8_t* sig96, size_t n, uint8_t out96[96]) {
     size_t nn = n ? n : 1;
-    Scratch* sc; if (int e = reserve(g.stream, nn * (96 + sizeof(g2a) + 1) + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* din = ar.take<uint8_t>(nn * 96); g2a* dpts = ar.take<g2a>(nn); uint8_t* dok = ar.take<uint8_t>(nn);
-    g2* dsum = ar.take<g2>(1); uint8_t* dout = ar.take<uint8_t>(96);
+    int err; const auto [din, dpts, dok, dsum, dout] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint8_t>(nn * 96), ar.take<g2a>(nn), ar.take<uint8_t>(nn), ar.take<g2>(1), ar.take<uint8_t>(96)};
+    });
+    if (err) return err;
     std::vector<uint8_t> ok(nn, 1);
     if (n) {
         CK(cudaMemcpyAsync(din, sig96, n * 96, cudaMemcpyHostToDevice, g.stream));
@@ -1340,15 +1349,15 @@ int hbls_aggregate_sigs(const uint8_t* sig96, size_t n, uint8_t out96[96]) {
 // B AggregateSig calls over n signature rows in HBM, shared by the host and device forms: every row decoded once, the sets summed by
 // chunks (kernels.cuh k_g2_segsum_*), the sums serialized into d_out96, the HBLS_AGG_* codes into d_status
 static size_t agg_batch_chunk_cap(size_t B, size_t n) { return (n + HB_AGG_CHUNK - 1) / HB_AGG_CHUNK + B; }
-static size_t agg_batch_scratch_bytes(size_t B, size_t n) {
-    return n * (sizeof(g2a) + 1) + agg_batch_chunk_cap(B, n) * (sizeof(g2) + 1 + 4) + (B + 1) * 8 + B * sizeof(g2) + 8 * 256;
+struct AggBatchBufs { g2a* pts; uint8_t* ok; uint64_t* first; uint32_t* chunk_set; g2* part; uint8_t* part_bad; g2* sum; };
+static AggBatchBufs carve_agg_batch(Arena& ar, size_t B, size_t n) {
+    const size_t cap = agg_batch_chunk_cap(B, n);
+    return {ar.take<g2a>(n), ar.take<uint8_t>(n), ar.take<uint64_t>(B + 1), ar.take<uint32_t>(cap), ar.take<g2>(cap), ar.take<uint8_t>(cap), ar.take<g2>(B)};
 }
 static void aggregate_sigs_batch_body(size_t B, size_t n, const uint64_t* d_offsets, const uint8_t* d_sigs96, uint8_t* d_out96, uint8_t* d_status,
-                                      cudaStream_t s, Arena& ar) {
+                                      cudaStream_t s, const AggBatchBufs& b) {
     const size_t cap = agg_batch_chunk_cap(B, n);
-    g2a* pts = ar.take<g2a>(n ? n : 1); uint8_t* ok = ar.take<uint8_t>(n ? n : 1);
-    uint64_t* first = ar.take<uint64_t>(B + 1); uint32_t* chunk_set = ar.take<uint32_t>(cap);
-    g2* part = ar.take<g2>(cap); uint8_t* part_bad = ar.take<uint8_t>(cap); g2* sum = ar.take<g2>(B);
+    const auto [pts, ok, first, chunk_set, part, part_bad, sum] = b;
     if (n) launch_g2_decode_checked(s, n, d_sigs96, pts, ok);
     LAUNCH(k_g2_segsum_plan, 1, HB_AGG_PLAN_THREADS, s, B, n, d_offsets, cap, first, chunk_set, d_status);
     LAUNCH(k_g2_segsum_chunks, blocks_for(32 * cap, 128), 128, s, B, (const uint64_t*)d_offsets, (const uint64_t*)first, (const uint32_t*)chunk_set,
@@ -1359,13 +1368,13 @@ static void aggregate_sigs_batch_body(size_t B, size_t n, const uint64_t* d_offs
 }
 static int aggregate_sigs_batch_locked(size_t B, const uint64_t* offsets, const uint8_t* sigs96, uint8_t* out96, uint8_t* status) {
     const size_t n = offsets[B];
-    Scratch* sc; if (int e = reserve(g.stream, agg_batch_scratch_bytes(B, n) + (B + 1) * 8 + n * 96 + B * 97 + 4 * 256, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint64_t* doff = ar.take<uint64_t>(B + 1); uint8_t* dsig = ar.take<uint8_t>(n ? 96 * n : 1);
-    uint8_t* dout = ar.take<uint8_t>(96 * B); uint8_t* dst = ar.take<uint8_t>(B);
+    int err; const auto [doff, dsig, dout, dst, bufs] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint64_t>(B + 1), ar.take<uint8_t>(96 * n), ar.take<uint8_t>(96 * B), ar.take<uint8_t>(B), carve_agg_batch(ar, B, n)};
+    });
+    if (err) return err;
     CK(cudaMemcpyAsync(doff, offsets, (B + 1) * 8, cudaMemcpyHostToDevice, g.stream));
     if (n) CK(cudaMemcpyAsync(dsig, sigs96, 96 * n, cudaMemcpyHostToDevice, g.stream));
-    aggregate_sigs_batch_body(B, n, doff, dsig, dout, dst, g.stream, ar);
+    aggregate_sigs_batch_body(B, n, doff, dsig, dout, dst, g.stream, bufs);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(out96, dout, 96 * B, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaMemcpyAsync(status, dst, B, cudaMemcpyDeviceToHost, g.stream));
@@ -1388,8 +1397,8 @@ int hbls_aggregate_sigs_batch_device(size_t B, size_t n, const void* d_offsets, 
         return HBLS_ERR_ARG;
     std::lock_guard<std::mutex> lk(g.mu);
     cudaStream_t s = stream ? (cudaStream_t)stream : g.stream;
-    return run_device_form(s, agg_batch_scratch_bytes(B, n), B, [&](Scratch*, Arena& ar) {
-        aggregate_sigs_batch_body(B, n, (const uint64_t*)d_offsets, (const uint8_t*)d_sigs96, (uint8_t*)d_out96, (uint8_t*)d_status, s, ar);
+    return run_device_form(s, B, [&](Arena& ar) { return carve_agg_batch(ar, B, n); }, [&](Scratch*, const AggBatchBufs& b) {
+        aggregate_sigs_batch_body(B, n, (const uint64_t*)d_offsets, (const uint8_t*)d_sigs96, (uint8_t*)d_out96, (uint8_t*)d_status, s, b);
     }, false);
 }
 
@@ -1401,45 +1410,41 @@ int hbls_aggregate_verify_batch_device(const hbls_committee* c, size_t B, const 
     if (B == 0) return 0;
     std::lock_guard<std::mutex> lk(g.mu);
     cudaStream_t s = stream ? (cudaStream_t)stream : g.stream;
-    return run_device_form(s, verify_scratch_bytes(B), B, [&](Scratch* sc, Arena& ar) {
-        agg_verify_device_locked(c, B, (const uint8_t*)d_bitmaps, blen, (const uint8_t*)d_sigs96, (const uint8_t*)d_msgs, msg_len, (uint8_t*)d_results, s, sc, ar, false);
+    return run_device_form(s, B, [&](Arena& ar) { return carve_verify(ar, B); }, [&](Scratch* sc, const VerifyBufs& v) {
+        agg_verify_device_locked(c, B, (const uint8_t*)d_bitmaps, blen, (const uint8_t*)d_sigs96, (const uint8_t*)d_msgs, msg_len, (uint8_t*)d_results, s, sc, v, false);
     });
 }
 // ------------------------------------------------------------------ bodies of the batch verifiers, shared by their host and device
-// forms: inputs in HBM, work enqueued on stream s in the scratch the caller reserved there, statuses computed on the device
+// forms: inputs in HBM, work enqueued on stream s in the buffers v = carve_verify(k) the caller carved, statuses computed on the device
 // (device_forms.cuh).  The H(m) hints are those launch_verify_tail takes: same_msg / h_msg from a host form (it sees the messages),
 // mg from a device form (messages grouped on the device).
 // triples: keys decoded on the device, verdicts into d_results; d_status (nullable) receives the HBLS_VB_* codes
 static void verify_triples_body(size_t k, const uint8_t* d_pk, const uint8_t* d_sig, const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results,
-                                uint8_t* d_status, cudaStream_t s, Scratch* sc, Arena& ar, bool same_msg, const MsgGroups* mg) {
-    VerifyBufs v = carve_verify(ar, k);
+                                uint8_t* d_status, cudaStream_t s, Scratch* sc, const VerifyBufs& v, bool same_msg, const MsgGroups* mg) {
     fork_point(k, sc, s);
     STAGE_EV(0, sc, s);
     // keys stay Jacobian (z = 1): the same tail as a mask aggregate, so independent triples also go through the batched groups
     LAUNCH(k_g1_decode_jac, heavy_blocks(k), TPB, s, k, d_pk, v.apk, v.ok_pk, 1);
     launch_verify_tail(k, v, sc, d_sig, d_msgs, (uint32_t)msg_len, v.ok_pk, d_results, s, same_msg, nullptr, mg);
     if (!d_status) return;
-    uint8_t* dflags = ar.take<uint8_t>(k);
-    LAUNCH(k_pack_flags, blocks_for(k, 256), 256, s, k, v.ok_sig, v.ok_hm, (const uint8_t*)v.ok_pk, dflags);
-    LAUNCH(k_status_triples, blocks_for(k, 256), 256, s, k, (const uint8_t*)dflags, (const uint8_t*)d_results, d_status);
+    LAUNCH(k_pack_flags, blocks_for(k, 256), 256, s, k, v.ok_sig, v.ok_hm, (const uint8_t*)v.ok_pk, v.flags);
+    LAUNCH(k_status_triples, blocks_for(k, 256), 256, s, k, (const uint8_t*)v.flags, (const uint8_t*)d_results, d_status);
 }
-// header ranges against one committee: HBLS_HDR_* codes into d_status
+// header ranges against one committee: verdicts into d_results, HBLS_HDR_* codes into d_status
 static void verify_headers_body(const hbls_committee* c, size_t n, const uint8_t* d_sigs, const uint8_t* d_bitmaps, size_t blen,
-                                const uint8_t* d_payloads, size_t payload_len, size_t quorum, uint8_t* d_status, cudaStream_t s, Scratch* sc,
-                                Arena& ar, bool same_msg, const uint8_t* h_msg, const MsgGroups* mg) {
-    uint8_t* dres = ar.take<uint8_t>(n); uint8_t* dflags = ar.take<uint8_t>(n);
-    VerifyBufs v;
-    agg_verify_device_locked(c, n, d_bitmaps, blen, d_sigs, d_payloads, payload_len, dres, s, sc, ar, same_msg, &v, h_msg, mg);
-    LAUNCH(k_pack_flags, blocks_for(n, 256), 256, s, n, v.ok_sig, v.ok_hm, (const uint8_t*)nullptr, dflags);
-    LAUNCH(k_status_headers, blocks_for(n, 256), 256, s, n, c->n, d_bitmaps, blen, quorum, (const uint8_t*)dflags, (const uint8_t*)dres, d_status);
+                                const uint8_t* d_payloads, size_t payload_len, size_t quorum, uint8_t* d_results, uint8_t* d_status, cudaStream_t s,
+                                Scratch* sc, const VerifyBufs& v, bool same_msg, const uint8_t* h_msg, const MsgGroups* mg) {
+    agg_verify_device_locked(c, n, d_bitmaps, blen, d_sigs, d_payloads, payload_len, d_results, s, sc, v, same_msg, h_msg, mg);
+    LAUNCH(k_pack_flags, blocks_for(n, 256), 256, s, n, v.ok_sig, v.ok_hm, (const uint8_t*)nullptr, v.flags);
+    LAUNCH(k_status_headers, blocks_for(n, 256), 256, s, n, c->n, d_bitmaps, blen, quorum, (const uint8_t*)v.flags, (const uint8_t*)d_results, d_status);
 }
-// items of a multi-committee batch (their bitmaps back to back in d_bitmaps): verdicts into d_results.  The descriptors (table,
-// bitmap, slots per item) come from the host array of handles.  They are written into the stream's own pinned buffer and uploaded
+// items of a multi-committee batch (their bitmaps back to back in d_bitmaps): verdicts into d_results, ditems = k descriptors (table,
+// bitmap, slots per item), which come from the host array of handles.  They are written into the stream's own pinned buffer and uploaded
 // with an asynchronous copy; an event recorded after that copy guards the buffer, so a later call on the same stream waits (on the
 // host) only if the earlier upload has not run yet.  A pageable copy would synchronise the stream.
 static int verify_items_body(size_t k, const hbls_committee* const* committees, const uint8_t* d_bitmaps, const uint8_t* d_sigs,
-                             const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, Arena& ar, bool same_msg,
-                             const MsgGroups* mg) {
+                             const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, const VerifyBufs& v,
+                             mask_item* ditems, bool same_msg, const MsgGroups* mg) {
     if (sc->items_pending) { CK(cudaEventSynchronize(sc->items_copied)); sc->items_pending = false; }
     if (!sc->items_copied) CK(cudaEventCreateWithFlags(&sc->items_copied, cudaEventDisableTiming));
     if (k > sc->h_items_cap) {
@@ -1448,8 +1453,6 @@ static int verify_items_body(size_t k, const hbls_committee* const* committees, 
         CK(cudaMallocHost(&sc->h_items, k * sizeof(mask_item)));
         sc->h_items_cap = k;
     }
-    VerifyBufs v = carve_verify(ar, k);
-    mask_item* ditems = ar.take<mask_item>(k);
     size_t off = 0;
     for (size_t j = 0; j < k; j++) {
         sc->h_items[j].table = committees[j]->table; sc->h_items[j].bitmap = d_bitmaps + off; sc->h_items[j].n = committees[j]->n;
@@ -1469,18 +1472,19 @@ static int verify_items_body(size_t k, const hbls_committee* const* committees, 
 // (hbls_verify_headers).  One message for all rounds: it keys the H(m) cache.
 static int agg_verify_host_locked(const hbls_committee* c, size_t B, const uint8_t* bitmaps, size_t blen, const uint8_t* sigs96,
                                   const uint8_t* msgs, size_t msg_len, uint8_t* out, bool status = false, size_t quorum = 0) {
-    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(B) + B * (blen + 96 + msg_len + 3) + 4096, &sc)) return e;
+    Scratch* sc; int err; const auto [dbm, dsig, dmsg, dout, dres, v] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint8_t>(B * blen), ar.take<uint8_t>(B * 96), ar.take<uint8_t>(B * msg_len), ar.take<uint8_t>(B),
+                          status ? ar.take<uint8_t>(B) : nullptr, carve_verify(ar, B)};       // dres: the verdicts behind the statuses
+    }, &sc);
+    if (err) return err;
     ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dbm = ar.take<uint8_t>(B * blen + 1); uint8_t* dsig = ar.take<uint8_t>(B * 96); uint8_t* dmsg = ar.take<uint8_t>(B * msg_len + 1);
-    uint8_t* dout = ar.take<uint8_t>(B);
     if (blen) CK(cudaMemcpyAsync(dbm, bitmaps, B * blen, cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(dsig, sigs96, B * 96, cudaMemcpyHostToDevice, g.stream));
     if (msg_len) CK(cudaMemcpyAsync(dmsg, msgs, B * msg_len, cudaMemcpyHostToDevice, g.stream));
     const bool same = all_messages_equal(msgs, B, msg_len);
     const uint8_t* h_msg = (same || B == 1) ? msgs : nullptr;
-    if (status) verify_headers_body(c, B, dsig, dbm, blen, dmsg, msg_len, quorum, dout, g.stream, sc, ar, same, h_msg, nullptr);
-    else agg_verify_device_locked(c, B, dbm, blen, dsig, dmsg, msg_len, dout, g.stream, sc, ar, same, nullptr, h_msg);
+    if (status) verify_headers_body(c, B, dsig, dbm, blen, dmsg, msg_len, quorum, dres, dout, g.stream, sc, v, same, h_msg, nullptr);
+    else agg_verify_device_locked(c, B, dbm, blen, dsig, dmsg, msg_len, dout, g.stream, sc, v, same, h_msg);
     CK(cudaMemcpyAsync(out, dout, B, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
     return 0;
@@ -1515,15 +1519,16 @@ static int aggregate_verify_items_locked(size_t k, const hbls_committee* const* 
                                 const uint8_t* msgs, size_t msg_len, uint8_t* results) {
     size_t bm_bytes = 0;
     for (size_t j = 0; j < k; j++) bm_bytes += (committees[j]->n + 7) >> 3;
-    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(k) + bm_bytes + k * (96 + msg_len + 1 + sizeof(mask_item)) + 4096, &sc)) return e;
+    Scratch* sc; int err; const auto [dbm, dsig, dmsg, dres, v, ditems] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint8_t>(bm_bytes), ar.take<uint8_t>(k * 96), ar.take<uint8_t>(k * msg_len), ar.take<uint8_t>(k),
+                          carve_verify(ar, k), ar.take<mask_item>(k)};
+    }, &sc);
+    if (err) return err;
     ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dbm = ar.take<uint8_t>(bm_bytes + 1); uint8_t* dsig = ar.take<uint8_t>(k * 96); uint8_t* dmsg = ar.take<uint8_t>(k * msg_len + 1);
-    uint8_t* dres = ar.take<uint8_t>(k);
     if (bm_bytes) CK(cudaMemcpyAsync(dbm, bitmaps, bm_bytes, cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(dsig, sigs96, k * 96, cudaMemcpyHostToDevice, g.stream));
     if (msg_len) CK(cudaMemcpyAsync(dmsg, msgs, k * msg_len, cudaMemcpyHostToDevice, g.stream));
-    if (int e = verify_items_body(k, committees, dbm, dsig, dmsg, msg_len, dres, g.stream, sc, ar, all_messages_equal(msgs, k, msg_len), nullptr)) return e;
+    if (int e = verify_items_body(k, committees, dbm, dsig, dmsg, msg_len, dres, g.stream, sc, v, ditems, all_messages_equal(msgs, k, msg_len), nullptr)) return e;
     CK(cudaMemcpyAsync(results, dres, k, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
     return 0;
@@ -1541,15 +1546,16 @@ int hbls_aggregate_verify_items(size_t k, const hbls_committee* const* committee
 // hbls_verify_batch: verdicts into out; with `status`, hbls_verify_batch_status: the caller learns WHY an item failed, in the order
 // the reference meets the errors (k_status_triples)
 static int verify_batch_locked(size_t k, const uint8_t* pk48, const uint8_t* sig96, const uint8_t* msgs, size_t msg_len, uint8_t* out, bool status) {
-    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(k) + k * (48 + 96 + msg_len + 3) + 4096, &sc)) return e;
+    Scratch* sc; int err; const auto [dpk, dsig, dmsg, dres, dst, v] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint8_t>(k * 48), ar.take<uint8_t>(k * 96), ar.take<uint8_t>(k * msg_len), ar.take<uint8_t>(k),
+                          status ? ar.take<uint8_t>(k) : nullptr, carve_verify(ar, k)};
+    }, &sc);
+    if (err) return err;
     ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dpk = ar.take<uint8_t>(k * 48); uint8_t* dsig = ar.take<uint8_t>(k * 96); uint8_t* dmsg = ar.take<uint8_t>(k * msg_len + 1);
-    uint8_t* dres = ar.take<uint8_t>(k); uint8_t* dst = status ? ar.take<uint8_t>(k) : nullptr;
     CK(cudaMemcpyAsync(dpk, pk48, k * 48, cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(dsig, sig96, k * 96, cudaMemcpyHostToDevice, g.stream));
     if (msg_len) CK(cudaMemcpyAsync(dmsg, msgs, k * msg_len, cudaMemcpyHostToDevice, g.stream));
-    verify_triples_body(k, dpk, dsig, dmsg, msg_len, dres, dst, g.stream, sc, ar, all_messages_equal(msgs, k, msg_len), nullptr);
+    verify_triples_body(k, dpk, dsig, dmsg, msg_len, dres, dst, g.stream, sc, v, all_messages_equal(msgs, k, msg_len), nullptr);
     CK(cudaMemcpyAsync(out, status ? dst : dres, k, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
     return 0;
@@ -1573,9 +1579,10 @@ int hbls_verify_batch_status(size_t k, const uint8_t* pk48, const uint8_t* sig96
 // the H(m) cache is neither read nor filled: the host never sees the messages)
 static int verify_batch_status_device_locked(size_t k, const uint8_t* d_pk, const uint8_t* d_sig, const uint8_t* d_msgs, size_t msg_len,
                                              uint8_t* d_status, cudaStream_t s) {
-    return run_device_form(s, verify_scratch_bytes(k) + group_bytes(k) + 2 * k + 4096, k, [&](Scratch* sc, Arena& ar) {
-        const MsgGroups mg = carve_groups(ar, k); uint8_t* dres = ar.take<uint8_t>(k);
-        verify_triples_body(k, d_pk, d_sig, d_msgs, msg_len, dres, d_status, s, sc, ar, false, &mg);
+    return run_device_form(s, k, [&](Arena& ar) { return std::tuple{carve_groups(ar, k), ar.take<uint8_t>(k), carve_verify(ar, k)}; },
+                           [&](Scratch* sc, const auto& b) {
+        const auto& [mg, dres, v] = b;
+        verify_triples_body(k, d_pk, d_sig, d_msgs, msg_len, dres, d_status, s, sc, v, false, &mg);
     });
 }
 int hbls_verify_batch_status_device(size_t k, const void* d_pk48, const void* d_sig96, const void* d_msgs, size_t msg_len, void* d_status, void* stream) {
@@ -1588,9 +1595,10 @@ int hbls_verify_batch_status_device(size_t k, const void* d_pk48, const void* d_
 }
 static int verify_headers_device_locked(const hbls_committee* c, size_t n, const uint8_t* d_sigs, const uint8_t* d_bitmaps, size_t blen,
                                         const uint8_t* d_payloads, size_t payload_len, size_t quorum, uint8_t* d_status, cudaStream_t s) {
-    return run_device_form(s, verify_scratch_bytes(n) + group_bytes(n) + 2 * n + 4096, n, [&](Scratch* sc, Arena& ar) {
-        const MsgGroups mg = carve_groups(ar, n);
-        verify_headers_body(c, n, d_sigs, d_bitmaps, blen, d_payloads, payload_len, quorum, d_status, s, sc, ar, false, nullptr, &mg);
+    return run_device_form(s, n, [&](Arena& ar) { return std::tuple{carve_groups(ar, n), ar.take<uint8_t>(n), carve_verify(ar, n)}; },
+                           [&](Scratch* sc, const auto& b) {
+        const auto& [mg, dres, v] = b;
+        verify_headers_body(c, n, d_sigs, d_bitmaps, blen, d_payloads, payload_len, quorum, dres, d_status, s, sc, v, false, nullptr, &mg);
     });
 }
 int hbls_verify_headers_device(const hbls_committee* c, size_t n, const void* d_sigs96, const void* d_bitmaps, size_t blen,
@@ -1604,11 +1612,10 @@ int hbls_verify_headers_device(const hbls_committee* c, size_t n, const void* d_
 }
 static int aggregate_verify_items_device_locked(size_t k, const hbls_committee* const* committees, const uint8_t* d_bitmaps, const uint8_t* d_sigs,
                                                 const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s) {
-    Scratch* sc; if (int e = reserve(s, verify_scratch_bytes(k) + group_bytes(k) + k * sizeof(mask_item) + 4096, &sc)) return e;
+    Scratch* sc; int err; const auto [mg, v, ditems] = carve_scratch(s, &err, [&](Arena& ar) { return std::tuple{carve_groups(ar, k), carve_verify(ar, k), ar.take<mask_item>(k)}; }, &sc);
+    if (err) return err;
     ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    const MsgGroups mg = carve_groups(ar, k);
-    if (int e = verify_items_body(k, committees, d_bitmaps, d_sigs, d_msgs, msg_len, d_results, s, sc, ar, false, &mg)) return e;
+    if (int e = verify_items_body(k, committees, d_bitmaps, d_sigs, d_msgs, msg_len, d_results, s, sc, v, ditems, false, &mg)) return e;
     CK(cudaGetLastError());
     return 0;
 }
@@ -1676,9 +1683,8 @@ int hbls_mask_get(const hbls_mask* m, uint8_t* bitmap_out, size_t blen, uint8_t 
     HostLock lk;
     if (bitmap_out) memcpy(bitmap_out, m->bitmap.data(), blen);
     if (pk48_out) {
-        Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
-        Arena ar{sc->base, 0, sc->cap};
-        uint8_t* dout = ar.take<uint8_t>(48);
+        int err; uint8_t* dout = carve_scratch(g.stream, &err, [](Arena& ar) { return ar.take<uint8_t>(48); });
+        if (err) return err;
         LAUNCH(k_g1_serialize, 1, 32, g.stream, (size_t)1, (const g1*)m->d_acc, dout);
         CK(cudaMemcpyAsync(pk48_out, dout, 48, cudaMemcpyDeviceToHost, g.stream));
         CK(cudaStreamSynchronize(g.stream));
@@ -1707,9 +1713,8 @@ static int ballot_box_add_vote_locked(hbls_ballot_box* b, const uint8_t* signer_
     const size_t n = b->c->n;
     for (size_t i = 0; i < n; i++)                                      // quorum.go:168-181: skip a ballot that shares a signer with a collected one
         if ((signer_bitmap[i >> 3] >> (i & 7)) & 1 && (b->collected[i >> 3] >> (i & 7)) & 1) return 1;
-    Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dsig = ar.take<uint8_t>(96); int* drc = ar.take<int>(1);
+    int err; const auto [dsig, drc] = carve_scratch(g.stream, &err, [](Arena& ar) { return std::tuple{ar.take<uint8_t>(96), ar.take<int>(1)}; });
+    if (err) return err;
     CK(cudaMemcpyAsync(dsig, sig96, 96, cudaMemcpyHostToDevice, g.stream));
     LAUNCH(k_single, 1, 32, g.stream, (size_t)1, (const single_desc*)nullptr, single_desc{dsig, nullptr, b->d_sum, OP_G2_DES_ADD, 0u}, drc);
     int rc = 0;
@@ -1732,20 +1737,20 @@ static_assert(HB_BALLOT_ACCEPTED == HBLS_BALLOT_ACCEPTED && HB_BALLOT_COLLECTED 
 // bitmap and the queue, one D2H copy of the statuses and the new bitmap, one synchronise.
 static int ballot_box_submit_votes_locked(hbls_ballot_box* b, size_t k, const uint8_t* signer_bitmaps, size_t blen, const uint8_t* sigs96,
                                           const void* msg, size_t msg_len, uint8_t* status) {
-    auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };            // the arena's alignment: offsets of the staged copy
-    const size_t o_sig = up(k * blen), o_col = o_sig + up(k * 96), o_msg = o_col + up(blen), in_bytes = o_msg + msg_len + 1;
-    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(k) + in_bytes + up(k + blen) + up(k) + 4096, &sc)) return e;
+    Arena in;                                                                // the staged copy: bitmaps, signatures, the box's bitmap, the message
+    const size_t o_bm = in.offset<uint8_t>(k * blen), o_sig = in.offset<uint8_t>(k * 96), o_col = in.offset<uint8_t>(blen), o_msg = in.offset<uint8_t>(msg_len);
+    Scratch* sc; int err; const auto [din, dres, dacc, dout, v] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint8_t>(in.off), ar.take<uint8_t>(k), ar.take<uint8_t>(k),
+                          ar.take<uint8_t>(k + blen), carve_verify(ar, k)};                // dout: statuses, then the new collected bitmap
+    }, &sc);
+    if (err) return err;
     ensure_stage_events(sc);
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* din = ar.take<uint8_t>(in_bytes); uint8_t* dres = ar.take<uint8_t>(k); uint8_t* dacc = ar.take<uint8_t>(k);
-    uint8_t* dout = ar.take<uint8_t>(k + blen);                             // statuses, then the new collected bitmap
-    std::vector<uint8_t> h(in_bytes, 0);
-    memcpy(h.data(), signer_bitmaps, k * blen); memcpy(h.data() + o_sig, sigs96, k * 96);
+    std::vector<uint8_t> h(in.off, 0);
+    memcpy(h.data() + o_bm, signer_bitmaps, k * blen); memcpy(h.data() + o_sig, sigs96, k * 96);
     memcpy(h.data() + o_col, b->collected.data(), blen); if (msg_len) memcpy(h.data() + o_msg, msg, msg_len);
-    CK(cudaMemcpyAsync(din, h.data(), in_bytes, cudaMemcpyHostToDevice, g.stream));
-    VerifyBufs v;
-    agg_verify_device_locked(b->c, k, din, blen, din + o_sig, din + o_msg, msg_len, dres, g.stream, sc, ar, true, &v, (const uint8_t*)msg);
-    LAUNCH(k_ballot_admit, 1, HB_BALLOT_THREADS, g.stream, k, b->c->n, blen, (const uint8_t*)din, (const uint8_t*)dres, (const uint8_t*)v.ok_sig,
+    CK(cudaMemcpyAsync(din, h.data(), in.off, cudaMemcpyHostToDevice, g.stream));
+    agg_verify_device_locked(b->c, k, din + o_bm, blen, din + o_sig, din + o_msg, msg_len, dres, g.stream, sc, v, true, (const uint8_t*)msg);
+    LAUNCH(k_ballot_admit, 1, HB_BALLOT_THREADS, g.stream, k, b->c->n, blen, (const uint8_t*)(din + o_bm), (const uint8_t*)dres, (const uint8_t*)v.ok_sig,
            (const uint8_t*)(din + o_col), dout + k, dout, dacc);
     LAUNCH(k_ballot_fold, 1, HB_SUM_THREADS, g.stream, k, (const g2a*)v.sig, (const uint8_t*)dacc, b->d_sum);
     std::vector<uint8_t> back(k + blen);
@@ -1765,9 +1770,8 @@ int hbls_ballot_box_submit_votes(hbls_ballot_box* b, size_t k, const uint8_t* si
     return ballot_box_submit_votes_locked(b, k, signer_bitmaps, blen, sigs96, msg, msg_len, status);
 }
 static int ballot_box_aggregate_locked(const hbls_ballot_box* b, uint8_t out_sig96[96], uint8_t* bitmap_out, size_t blen) {
-    Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dout = ar.take<uint8_t>(96);
+    int err; uint8_t* dout = carve_scratch(g.stream, &err, [](Arena& ar) { return ar.take<uint8_t>(96); });
+    if (err) return err;
     LAUNCH(k_g2_serialize, 1, 32, g.stream, (size_t)1, (const g2*)b->d_sum, dout);
     CK(cudaMemcpyAsync(out_sig96, dout, 96, cudaMemcpyDeviceToHost, g.stream));
     CK(cudaStreamSynchronize(g.stream));
@@ -1789,11 +1793,11 @@ static int rlc_partial_locked(size_t k, const uint8_t* pk48, const uint8_t* sig9
     PartialRecord rec; memset(&rec, 0, sizeof rec);
     const size_t kk = k ? k : 1;
     const unsigned W = (unsigned)(kk < (size_t)g.sm_count * 2 ? kk : (size_t)g.sm_count * 2);      // warps that multiply Miller values into partial products
-    Scratch* sc; if (int e = reserve(g.stream, verify_scratch_bytes(kk) + kk * (48 + 96 + msg_len + 8) + (W + 2) * 6 * sizeof(fp2) + sizeof(g2) + 8192, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    VerifyBufs v = carve_verify(ar, kk);
-    uint8_t* dpk = ar.take<uint8_t>(kk * 48); uint8_t* dsig = ar.take<uint8_t>(kk * 96); uint8_t* dmsg = ar.take<uint8_t>(kk * msg_len + 1);
-    uint64_t* dco = ar.take<uint64_t>(kk); fp2* dpart = ar.take<fp2>((size_t)W * 6); fp2* dprod = ar.take<fp2>(6); g2* dS = ar.take<g2>(1);
+    int err; const auto [v, dpk, dsig, dmsg, dco, dpart, dprod, dS] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{carve_verify(ar, kk), ar.take<uint8_t>(kk * 48), ar.take<uint8_t>(kk * 96), ar.take<uint8_t>(kk * msg_len),
+                          ar.take<uint64_t>(kk), ar.take<fp2>((size_t)W * 6), ar.take<fp2>(6), ar.take<g2>(1)};
+    });
+    if (err) return err;
     if (k) {
         const std::vector<uint64_t> co = rlc_draw_items(k);
         CK(cudaMemcpyAsync(dpk, pk48, k * 48, cudaMemcpyHostToDevice, g.stream));
@@ -1829,9 +1833,10 @@ int hbls_rlc_partial(size_t k, const uint8_t* pk48, const uint8_t* sig96, const 
 }
 // the device part of hbls_rlc_fold (records that hold items and no undecodable one)
 static int rlc_fold_locked(size_t n, const uint8_t* records) {
-    Scratch* sc; if (int e = reserve(g.stream, n * (sizeof(g2) + 6 * sizeof(fp2)) + sizeof(g2) + sizeof(g2a) + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    g2* dS = ar.take<g2>(n); fp2* dparts = ar.take<fp2>(n * 6); g2* dsum = ar.take<g2>(1); g2a* dsg = ar.take<g2a>(1); uint8_t* dres = ar.take<uint8_t>(1);
+    int err; const auto [dS, dparts, dsum, dsg, dres] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<g2>(n), ar.take<fp2>(n * 6), ar.take<g2>(1), ar.take<g2a>(1), ar.take<uint8_t>(1)};
+    });
+    if (err) return err;
     std::vector<g2> hs(n); std::vector<fp2> hf(n * 6);
     for (size_t p = 0; p < n; p++) { PartialRecord r; memcpy(&r, records + p * HBLS_PARTIAL_BYTES, HBLS_PARTIAL_BYTES); hs[p] = r.S; for (int i = 0; i < 6; i++) hf[6 * p + i] = r.f[i]; }
     CK(cudaMemcpyAsync(dS, hs.data(), n * sizeof(g2), cudaMemcpyHostToDevice, g.stream));
@@ -1855,10 +1860,10 @@ int hbls_rlc_fold(size_t n, const uint8_t* records) {
 }
 
 static int sign_hash_batch_locked(size_t k, const uint8_t* sk32, const uint8_t* msgs, size_t msg_len, uint8_t* sig96_out, uint8_t* ok) {
-    Scratch* sc; if (int e = reserve(g.stream, k * (32 + msg_len + sizeof(g2) + 96 + 1) + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dsk = ar.take<uint8_t>(k * 32); uint8_t* dmsg = ar.take<uint8_t>(k * msg_len + 1); g2* dpts = ar.take<g2>(k);
-    uint8_t* dout = ar.take<uint8_t>(k * 96); uint8_t* dok = ar.take<uint8_t>(k);
+    int err; const auto [dsk, dmsg, dpts, dout, dok] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint8_t>(k * 32), ar.take<uint8_t>(k * msg_len), ar.take<g2>(k), ar.take<uint8_t>(k * 96), ar.take<uint8_t>(k)};
+    });
+    if (err) return err;
     CK(cudaMemcpyAsync(dsk, sk32, k * 32, cudaMemcpyHostToDevice, g.stream));
     if (msg_len) CK(cudaMemcpyAsync(dmsg, msgs, k * msg_len, cudaMemcpyHostToDevice, g.stream));
     LAUNCH(k_sign_hash, blocks_for(k, TPB), TPB, g.stream, k, dsk, dmsg, (uint32_t)msg_len, dpts, dok);
@@ -1903,54 +1908,38 @@ static int sign_hash_keys_locked(size_t k, const uint8_t* sk32, size_t m, const 
     }
     const size_t nf = fit.size(), nb = big.size(), per_msg = nf + (agg ? 1 : 0);
     const size_t ngls = m * per_msg, npair = m * nb, N = ngls + npair;
-    // H(m): one table entry per distinct message, misses at the front (one hash launch), cached entries at the back (as part1_locked)
-    std::vector<std::array<uint8_t, 48>> keys; std::vector<uint32_t> msg_entry(m);
-    {
-        std::map<std::array<uint8_t, 48>, uint32_t> seen;
-        for (size_t j = 0; j < m; j++) {
-            std::array<uint8_t, 48> key; hm_key(key.data(), msg_len ? msgs + j * msg_len : nullptr, msg_len);
-            auto it = seen.emplace(key, (uint32_t)keys.size());
-            if (it.second) keys.push_back(key);
-            msg_entry[j] = it.first->second;
-        }
-    }
-    const size_t nk = keys.size();
-    std::vector<uint32_t> pos(nk); std::vector<bool> cached(nk, false); size_t nmiss = 0;
-    for (size_t d = 0; d < nk; d++) cached[d] = hm_enabled() && hm_find(keys[d].data()) >= 0;
-    for (size_t d = 0, hit = 0; d < nk; d++) pos[d] = cached[d] ? (uint32_t)(nk - 1 - hit++) : (uint32_t)nmiss++;
+    // H(m): hm_tab.entry[j] = table entry of message j
+    const HmTable hm_tab = hm_table(m, [&](size_t j) { return std::pair{msg_len ? msgs + j * msg_len : nullptr, msg_len}; });
+    const size_t nk = hm_tab.keys.size();
     // one distinct message: every item reads entry 0 (stride 0); else each item gets its message's point by k_broadcast_hm
     const bool gather = nk > 1;
     auto item_msg = [&](size_t i) { return i < ngls ? i / per_msg : (i - ngls) / nb; };
-    Layout in, out;
-    const size_t i_keys = in.put(nmiss * 48), i_idx = gather ? in.put(N * 4) : 0, i_dig = in.put(ngls * 32), i_sk = in.put(npair * 32);
-    const size_t o_ser = out.put(N * 96), o_ok = out.put(N);
-    Scratch* sc;
-    if (int e = reserve(s, in.size + out.size + (nk + (gather ? N : 0)) * (sizeof(g2a) + 1) + N * sizeof(g2) + 8 * 256, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* din = ar.take<uint8_t>(in.size); uint8_t* dout = ar.take<uint8_t>(out.size);
-    g2a* th = ar.take<g2a>(nk); uint8_t* tok = ar.take<uint8_t>(nk);
-    g2a* hm = gather ? ar.take<g2a>(N) : th; uint8_t* ok_hm = gather ? ar.take<uint8_t>(N) : tok;
-    g2* dsig = ar.take<g2>(N);
-    std::vector<uint8_t> hin(in.size), hout(out.size);
+    Arena in, out;
+    const size_t i_keys = in.offset<uint8_t>(hm_tab.nmiss * 48), i_idx = gather ? in.offset<uint32_t>(N) : 0, i_dig = in.offset<uint8_t>(ngls * 32);
+    const size_t i_sk = in.offset<uint8_t>(npair * 32);
+    const size_t o_ser = out.offset<uint8_t>(N * 96), o_ok = out.offset<uint8_t>(N);
+    int err; const auto [din, dout, th, tok, hm, ok_hm, dsig] = carve_scratch(s, &err, [&](Arena& ar) {
+        uint8_t* din = ar.take<uint8_t>(in.off); uint8_t* dout = ar.take<uint8_t>(out.off);
+        g2a* th = ar.take<g2a>(nk); uint8_t* tok = ar.take<uint8_t>(nk);
+        g2a* hm = gather ? ar.take<g2a>(N) : th; uint8_t* ok_hm = gather ? ar.take<uint8_t>(N) : tok;
+        return std::tuple{din, dout, th, tok, hm, ok_hm, ar.take<g2>(N)};
+    });
+    if (err) return err;
+    std::vector<uint8_t> hin(in.off), hout(out.off);
     // the digit and key sections are adjacent: [key_lo, key_hi) holds every secret byte of the staging copy.  The host copy is wiped on
     // every return path, the device copy on the stream after the ladder kernels.
     const size_t key_lo = i_dig, key_hi = i_sk + npair * 32;
     struct WipeKeys { uint8_t* p; size_t n; ~WipeKeys() { hb_secret::wipe(p, n); } } wipe_keys{hin.data() + key_lo, key_hi - key_lo};
-    for (size_t d = 0; d < nk; d++) if (!cached[d]) memcpy(&hin[i_keys + 48 * pos[d]], keys[d].data(), 48);
-    if (gather) for (size_t i = 0; i < N; i++) { const uint32_t e = pos[msg_entry[item_msg(i)]]; memcpy(&hin[i_idx + 4 * i], &e, 4); }
+    hm_tab.stage_misses(&hin[i_keys]);
+    if (gather) for (size_t i = 0; i < N; i++) memcpy(&hin[i_idx + 4 * i], &hm_tab.entry[item_msg(i)], 4);
     for (size_t j = 0; j < m; j++) {
         uint8_t* dg = &hin[i_dig + 32 * j * per_msg];
         for (size_t r = 0; r < nf; r++) memcpy(dg + 32 * r, &kd[4 * fit[r]], 32);
         if (agg) memcpy(dg + 32 * nf, &kd[4 * k], 32);
         for (size_t r = 0; r < nb; r++) memcpy(&hin[i_sk + 32 * (j * nb + r)], sk32 + 32 * big[r], 32);
     }
-    CK(cudaMemcpyAsync(din, hin.data(), in.size, cudaMemcpyHostToDevice, s));
-    for (size_t d = 0; d < nk; d++) if (cached[d]) hm_fetch(keys[d].data(), th + pos[d], tok + pos[d], s);
-    if (hm_enabled()) g.hm_misses += nmiss;
-    if (nmiss) {
-        launch_hash_small(s, nmiss, din + i_keys, 48, th, tok);
-        if (hm_enabled()) for (size_t d = 0; d < nk; d++) if (!cached[d]) hm_store(keys[d].data(), th + pos[d], tok + pos[d], s);
-    }
+    CK(cudaMemcpyAsync(din, hin.data(), in.off, cudaMemcpyHostToDevice, s));
+    hm_table_fill(hm_tab, din + i_keys, th, tok, s);
     if (gather) LAUNCH(k_broadcast_hm, blocks_for(N, 256), 256, s, N, (const uint32_t*)(din + i_idx), (const g2a*)th, (const uint8_t*)tok, hm, ok_hm);
     const size_t stride = gather ? 1 : 0;
     uint8_t* dok = dout + o_ok;
@@ -1960,7 +1949,7 @@ static int sign_hash_keys_locked(size_t k, const uint8_t* sk32, size_t m, const 
     CK(cudaMemsetAsync(din + key_lo, 0, key_hi - key_lo, s));
     LAUNCH(k_g2_serialize, blocks_for(N, TPB), TPB, s, N, (const g2*)dsig, dout + o_ser);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(hout.data(), dout, out.size, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(hout.data(), dout, out.off, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     for (size_t i = 0; i < N; i++) {
         const size_t j = item_msg(i);
@@ -1985,9 +1974,10 @@ int hbls_sign_hash_keys(size_t k, const uint8_t* sk32, size_t m, const uint8_t* 
     return sign_hash_keys_locked(k, sk32, m, msgs, msg_len, sigs96, aggs96, ok);
 }
 static int get_public_key_batch_locked(size_t k, const uint8_t* sk32, uint8_t* pk48_out) {
-    Scratch* sc; if (int e = reserve(g.stream, k * (32 + sizeof(g1) + 48) + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* dsk = ar.take<uint8_t>(k * 32); g1* dpts = ar.take<g1>(k); uint8_t* dout = ar.take<uint8_t>(k * 48);
+    int err; const auto [dsk, dpts, dout] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint8_t>(k * 32), ar.take<g1>(k), ar.take<uint8_t>(k * 48)};
+    });
+    if (err) return err;
     CK(cudaMemcpyAsync(dsk, sk32, k * 32, cudaMemcpyHostToDevice, g.stream));
     LAUNCH(k_g1_mul_gen, blocks_for(k, TPB), TPB, g.stream, k, dsk, dpts);
     CK(cudaMemsetAsync(dsk, 0, k * 32, g.stream));
@@ -2004,9 +1994,10 @@ int hbls_get_public_key_batch(size_t k, const uint8_t* sk32, uint8_t* pk48_out) 
 }
 
 static int fp_mul_batch_locked(size_t n, const uint8_t* a48, const uint8_t* b48, uint8_t* out48) {
-    Scratch* sc; if (int e = reserve(g.stream, n * 144 + 4096, &sc)) return e;
-    Arena ar{sc->base, 0, sc->cap};
-    uint8_t* da = ar.take<uint8_t>(n * 48); uint8_t* db = ar.take<uint8_t>(n * 48); uint8_t* dout = ar.take<uint8_t>(n * 48);
+    int err; const auto [da, db, dout] = carve_scratch(g.stream, &err, [&](Arena& ar) {
+        return std::tuple{ar.take<uint8_t>(n * 48), ar.take<uint8_t>(n * 48), ar.take<uint8_t>(n * 48)};
+    });
+    if (err) return err;
     CK(cudaMemcpyAsync(da, a48, n * 48, cudaMemcpyHostToDevice, g.stream));
     CK(cudaMemcpyAsync(db, b48, n * 48, cudaMemcpyHostToDevice, g.stream));
     LAUNCH(k_fp_mul, blocks_for(n, 128), 128, g.stream, n, da, db, dout);
@@ -2037,8 +2028,8 @@ int hbls_stage_timing_get(float* ms_out, int max_stages) {
     return n;
 }
 static int selftest_split_locked(uint32_t iters) {
-    Scratch* sc; if (int e = reserve(g.stream, 4096, &sc)) return e;
-    uint32_t* d = reinterpret_cast<uint32_t*>(sc->base);
+    int err; uint32_t* d = carve_scratch(g.stream, &err, [](Arena& ar) { return ar.take<uint32_t>(1); });
+    if (err) return err;
     CK(cudaMemsetAsync(d, 0, 4, g.stream));
     LAUNCH(k_selftest_fp2h, 8, 64, g.stream, iters, 20240922u, d);
     uint32_t bad = 0;
@@ -2054,9 +2045,8 @@ int hbls_selftest_split(uint32_t iters) {
 double hbls_probe_mac32_per_s(int iters, double* sm_clock_hz) {
     if (ensure_init()) return -1.0;
     HostLock lk;
-    Scratch* sc; if (reserve(g.stream, 4096, &sc)) return -1.0;
-    uint32_t* sink = reinterpret_cast<uint32_t*>(sc->base);
-    unsigned long long* cyc = reinterpret_cast<unsigned long long*>(sc->base + 256);
+    int err; const auto [sink, cyc] = carve_scratch(g.stream, &err, [](Arena& ar) { return std::tuple{ar.take<uint32_t>(1), ar.take<unsigned long long>(1)}; });
+    if (err) return -1.0;
     constexpr int K = 4;
     const int threads = 256, blocks = g.sm_count * 2;                  // one wave: 2 x 256 threads x 94 registers per SM
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
