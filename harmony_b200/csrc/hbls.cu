@@ -209,9 +209,19 @@ unsigned capped_blocks(size_t n, long long tpsm, unsigned tpb) {
 }
 unsigned heavy_blocks(size_t n) { return capped_blocks(n, g.tpsm, TPB); }
 unsigned light_blocks(size_t n) { return capped_blocks(n, g.tpsm_light, TPB); }       // small-state kernels: the register count decides
-unsigned split_blocks(size_t nthreads) { return capped_blocks(nthreads, g.tpsm_split, HB_TPB_SPLIT); }
 // lock-stepped lane-pair kernels: one CTA per SM, its size = the resident threads wanted for that kernel (multiple of 64, <= 512)
 unsigned lockstep_cta(long long t) { t = t < 64 ? 64 : (t > HB_TPB_SPLIT ? HB_TPB_SPLIT : t); return (unsigned)(t & ~63ll); }
+// n lane pairs give every SM a full CTA of HB_TPB_SPLIT threads
+bool fills_chip(size_t n) { return 2 * n >= (size_t)g.sm_count * HB_TPB_SPLIT; }
+// lane-pair kernels over n threads: a batch that fills the chip runs on CTAs of `cta` threads, at most `tpsm` resident threads per SM
+// (by default HB_TPB_SPLIT and tpsm_split; a lock-stepped kernel passes its lockstep_cta as both: one CTA per SM), a smaller one on
+// 64-thread CTAs spread over the SMs
+struct Geom { unsigned grid, cta; };
+Geom pair_geom(size_t n, bool full, unsigned cta = HB_TPB_SPLIT, long long tpsm = g.tpsm_split) {
+    return full ? Geom{capped_blocks(n, tpsm, cta), cta} : Geom{blocks_for(n, 64), 64};
+}
+// warp-per-round kernels over n items: at most coop_wpsm resident warps per SM
+unsigned coop_blocks(size_t n) { const size_t cap = (size_t)g.sm_count * (size_t)(g.coop_wpsm > 0 ? g.coop_wpsm : 1); return (unsigned)(n < cap ? n : cap); }
 
 // signature decode of a large batch, one signature per thread: the subgroup test inside the decode, or (decode_split) as a
 // lane-pair kernel after it; a point outside G2 is zeroed and loses its ok flag either way
@@ -280,49 +290,12 @@ std::vector<uint64_t> rlc_draw_items(size_t k) {
 // batched form: groups of 8 once that still gives every SM a full CTA of lane pairs (fewer Miller-loop pairs and final exponentiations
 // per round), else 4
 size_t rlc_group_size(size_t B) {
-    return (g.rlc_g == 4 || g.rlc_g == 8) ? (size_t)g.rlc_g : (2 * (B / 8) >= (size_t)g.sm_count * HB_TPB_SPLIT ? 8 : 4);
+    return (g.rlc_g == 4 || g.rlc_g == 8) ? (size_t)g.rlc_g : (fills_chip(B / 8) ? 8 : 4);
 }
 // two-phase form: groups per pass = one lane pair per group on every SM (256 lane pairs per SM), i.e. one wave of the line kernel
 size_t rlc_chunk_groups() { return (size_t)g.sm_count * (HB_TPB_SPLIT / 2); }
-static bool rlc_applies(size_t B);
-static bool exact_two_phase(size_t B);
-size_t rlc_lines_bytes(size_t B) {
-    if (!g.rlc_two_phase) return 0;
-    if (!rlc_applies(B)) {      // exact form through the same kernels: "groups" of one round, two pairs each
-        if (!exact_two_phase(B)) return 0;
-        const size_t ngc = B < rlc_chunk_groups() ? B : rlc_chunk_groups();
-        return (size_t)HB_ML_STEPS * 3 * 2 * ngc * 2 * sizeof(fp) + 256;
-    }
-    const size_t G = rlc_group_size(B), ng = B / G, ngc = ng < rlc_chunk_groups() ? ng : rlc_chunk_groups();
-    const size_t rlc_bytes = (size_t)HB_ML_STEPS * 3 * (G + 1) * ngc * 2 * sizeof(fp);
-    // the exact pass over the rounds of failed groups runs through the same buffer ("groups" of one round, <= all rounds of the batch)
-    const size_t nlc = B < rlc_chunk_groups() ? B : rlc_chunk_groups();
-    const size_t list_bytes = g.exact_two_phase ? (size_t)HB_ML_STEPS * 3 * 2 * nlc * 2 * sizeof(fp) + B * sizeof(g2a) + 256 : 0;
-    return (rlc_bytes > list_bytes ? rlc_bytes : list_bytes) + 256;
-}
 // blocks per call at most: S <= ceil(ng / HB_RLC_M) + 31
 size_t rlc_nblocks_max(size_t B) { return B / HB_RLC_G / HB_RLC_M + 32; }
-// flags: the packed decode flags of the status forms (k_pack_flags)
-struct VerifyBufs { g2a* sig; g2a* hm; g1a* pkneg; g1* apk; uint8_t* ok_sig; uint8_t* ok_hm; uint8_t* ok_pk;
-                    g1a* pk_scaled; g2* S; uint8_t* bad; g2a* Sg; uint8_t* group_ok; uint32_t* fail_list; unsigned* counts; g2a* Sb; uint8_t* block_ok;
-                    fp2* f1; uint8_t* irr1; fp2* f2; uint8_t* irr2; uint8_t* ok_sub;
-                    uint16_t* mask_cost; unsigned* mask_hist; uint32_t* mask_order; fp* lines; uint8_t* verdict; uint8_t* flags; };
-VerifyBufs carve_verify(Arena& ar, size_t B) {
-    VerifyBufs v;
-    v.sig = ar.take<g2a>(B); v.hm = ar.take<g2a>(B); v.pkneg = ar.take<g1a>(B); v.apk = ar.take<g1>(B);
-    v.ok_sig = ar.take<uint8_t>(B); v.ok_hm = ar.take<uint8_t>(B); v.ok_pk = ar.take<uint8_t>(B);
-    v.pk_scaled = ar.take<g1a>(B); v.S = ar.take<g2>(B); v.bad = ar.take<uint8_t>(B);
-    v.Sg = ar.take<g2a>(B / HB_RLC_G + 1); v.group_ok = ar.take<uint8_t>(B / HB_RLC_G + 1);
-    v.fail_list = ar.take<uint32_t>(B); v.counts = ar.take<unsigned>(5);      // [0] [1] k_rlc_finish, [2] [3] form gates, [4] per-group check list
-    v.Sb = ar.take<g2a>(rlc_nblocks_max(B)); v.block_ok = ar.take<uint8_t>(rlc_nblocks_max(B));
-    v.mask_cost = ar.take<uint16_t>(B); v.mask_hist = ar.take<unsigned>(HB_MASK_BINS); v.mask_order = ar.take<uint32_t>(B);
-    v.verdict = ar.take<uint8_t>(B); v.flags = ar.take<uint8_t>(B);
-    v.lines = nullptr;
-    if (rlc_lines_bytes(B)) v.lines = reinterpret_cast<fp*>(ar.take<uint8_t>(rlc_lines_bytes(B)));
-    v.f1 = v.f2 = nullptr; v.irr1 = v.irr2 = v.ok_sub = nullptr;
-    if (B <= 8192) { v.f1 = ar.take<fp2>(6 * B); v.irr1 = ar.take<uint8_t>(B); v.f2 = ar.take<fp2>(6 * B); v.irr2 = ar.take<uint8_t>(B); v.ok_sub = ar.take<uint8_t>(B); }
-    return v;
-}
 // Small batches (latency path): the inputs are on the device from here on -- signature decode and hash-to-G2 may start on the
 // auxiliary streams while the caller's stream still aggregates the public keys (launch_verify_tail joins them before the pairing).
 static bool latency_path(size_t B);
@@ -333,6 +306,9 @@ void fork_point(size_t B, Scratch* sc, cudaStream_t s) {
 // batched (random-linear-combination) form applies: default mode and a batch large enough
 static bool rlc_applies(size_t B) { return g.batch_mode == 1 && (long long)B >= g.rlc_min && B >= 2 * HB_RLC_GMAX; }
 static bool latency_path(size_t B) { return !rlc_applies(B) && (long long)B <= g.coop_max; }
+// the pairing of the batched form's ng groups runs as line kernel + accumulator kernel: rlc_two_phase 1 once the groups fill the
+// chip, 2 always
+static bool rlc_groups_two_phase(size_t ng) { return g.rlc_two_phase && (fills_chip(ng) || g.rlc_two_phase >= 2); }
 // blocks of HB_RLC_M groups share one final exponentiation and one generator pair (kernels.cuh: rlc_block_coeffs).  They need the
 // two-kernel pairing with every group in ONE chunk of the line buffer (a block must not span chunks); automatically from one whole
 // block on, rlc_block = 1 / 2 forces them on / off (wherever they can run at all)
@@ -340,14 +316,65 @@ static bool rlc_blocks(size_t ng, bool two_phase) {
     if (!two_phase || g.rlc_block == 2 || ng > rlc_chunk_groups()) return false;
     return g.rlc_block == 1 || ng >= HB_RLC_M;
 }
-// the groups' Miller values of the block form: 6 Fp2 per group, behind the G round pairs' lines (the buffer holds G + 1 pairs)
-static fp2* rlc_fm(const VerifyBufs& v, size_t G, size_t ng) { return reinterpret_cast<fp2*>(v.lines + (size_t)HB_ML_STEPS * 3 * G * ng * 2); }
 // exact checks of batches beyond the warp-per-round range run as line kernel + accumulator kernel too (twice the lane pairs in the
 // first one; the second no longer carries the running points)
 static bool exact_two_phase(size_t B) { return g.rlc_two_phase >= 2 && g.exact_two_phase && !rlc_applies(B) && (long long)B > g.coop_max; }
-// exact check of n rounds (contiguous arrays) as "groups" of one round through k_rlc_lines_split<1> / k_rlc_accum_split<1>
+// flags: the packed decode flags of the status forms (k_pack_flags).  The line buffer (null where no two-kernel pairing runs):
+// lines / fm, the group pass's lines and the block form's Miller values; ex_lines / ex_hm over the same bytes, the lines of the exact
+// two-kernel pass and the H(m) it gathers for the failed groups' rounds (launch_exact_two_phase)
+struct VerifyBufs { g2a* sig; g2a* hm; g1a* pkneg; g1* apk; uint8_t* ok_sig; uint8_t* ok_hm; uint8_t* ok_pk;
+                    g1a* pk_scaled; g2* S; uint8_t* bad; g2a* Sg; uint8_t* group_ok; uint32_t* fail_list; unsigned* counts; g2a* Sb; uint8_t* block_ok;
+                    fp2* f1; uint8_t* irr1; fp2* f2; uint8_t* irr2; uint8_t* ok_sub;
+                    uint16_t* mask_cost; unsigned* mask_hist; uint32_t* mask_order; fp* lines; fp2* fm; fp* ex_lines; g2a* ex_hm; uint8_t* verdict;
+                    uint8_t* flags; };
+VerifyBufs carve_verify(Arena& ar, size_t B) {
+    VerifyBufs v{};
+    v.sig = ar.take<g2a>(B); v.hm = ar.take<g2a>(B); v.pkneg = ar.take<g1a>(B); v.apk = ar.take<g1>(B);
+    v.ok_sig = ar.take<uint8_t>(B); v.ok_hm = ar.take<uint8_t>(B); v.ok_pk = ar.take<uint8_t>(B);
+    v.pk_scaled = ar.take<g1a>(B); v.S = ar.take<g2>(B); v.bad = ar.take<uint8_t>(B);
+    v.Sg = ar.take<g2a>(B / HB_RLC_G + 1); v.group_ok = ar.take<uint8_t>(B / HB_RLC_G + 1);
+    v.fail_list = ar.take<uint32_t>(B); v.counts = ar.take<unsigned>(5);      // [0] [1] k_rlc_finish, [2] [3] form gates, [4] per-group check list
+    v.Sb = ar.take<g2a>(rlc_nblocks_max(B)); v.block_ok = ar.take<uint8_t>(rlc_nblocks_max(B));
+    v.mask_cost = ar.take<uint16_t>(B); v.mask_hist = ar.take<unsigned>(HB_MASK_BINS); v.mask_order = ar.take<uint32_t>(B);
+    v.verdict = ar.take<uint8_t>(B); v.flags = ar.take<uint8_t>(B);
+    // the line buffer: one region of the larger of two layouts.  The exact pass over the failed groups' rounds runs behind the group
+    // pass on the same stream, so it may overwrite the group pass's lines and Miller values.  Lines are per chunk of groups.
+    const size_t G = rlc_group_size(B), ng = B / G, W = rlc_chunk_groups();
+    const bool groups = rlc_applies(B) && rlc_groups_two_phase(ng), exact = (groups && g.exact_two_phase) || exact_two_phase(B);
+    auto group_layout = [&](Arena& a) {
+        if (!groups) return;
+        v.lines = a.take<fp>((size_t)HB_ML_STEPS * 3 * (G + 1) * std::min(ng, W) * 2);      // G + 1 pairs per group
+        if (rlc_blocks(ng, true)) v.fm = a.take<fp2>(6 * ng);
+    };
+    auto exact_layout = [&](Arena& a) {
+        if (!exact) return;
+        v.ex_lines = a.take<fp>((size_t)HB_ML_STEPS * 3 * 2 * std::min(B, W) * 2);           // 2 pairs per round
+        if (groups) v.ex_hm = a.take<g2a>(B);
+    };
+    if (const size_t bytes = std::max(Arena::bytes(group_layout), Arena::bytes(exact_layout))) {
+        Arena region{(uintptr_t)ar.take<uint8_t>(bytes)}, again = region;
+        group_layout(region); exact_layout(again);
+    }
+    if (B <= 8192) { v.f1 = ar.take<fp2>(6 * B); v.irr1 = ar.take<uint8_t>(B); v.f2 = ar.take<fp2>(6 * B); v.irr2 = ar.take<uint8_t>(B); v.ok_sub = ar.take<uint8_t>(B); }
+    return v;
+}
+// exact check of n rounds as "groups" of one round through k_rlc_lines_split<1> / k_rlc_accum_split<1>: the rounds of the contiguous
+// arrays, or with idx / count (the failed groups' list, counted on the device) the listed rounds, which k_exact_prepare gathers into
+// pk_c / hm_c / sig_c; the launches are then sized for n and return at once beyond the count
 void launch_exact_two_phase(size_t n, const g2a* sig, const g1a* pkneg, const g2a* hm, const uint8_t* ok_a, const uint8_t* ok_b, const uint8_t* ok_c,
-                            uint8_t* bad, uint8_t* verdict, fp* lines, uint8_t* d_results, cudaStream_t s);
+                            uint8_t* bad, uint8_t* verdict, fp* lines, uint8_t* d_results, cudaStream_t s, const uint32_t* idx = nullptr,
+                            const unsigned* count = nullptr, g1a* pk_c = nullptr, g2a* hm_c = nullptr, g2a* sig_c = nullptr) {
+    LAUNCH(k_exact_prepare, blocks_for(n, 256), 256, s, n, idx, sig, pkneg, hm, ok_a, ok_b, ok_c, pk_c, hm_c, sig_c, bad, d_results, count);
+    if (idx) { pkneg = pk_c; hm = hm_c; sig = sig_c; }
+    const bool full = fills_chip(n);
+    for (size_t g0 = 0; g0 < n; g0 += rlc_chunk_groups()) {
+        const size_t nc = n - g0 < rlc_chunk_groups() ? n - g0 : rlc_chunk_groups();
+        const Geom lg = pair_geom(4 * nc, full), ag = pair_geom(2 * nc, full);
+        LAUNCH(k_rlc_lines_split<1>, lg.grid, lg.cta, s, n, g0, nc, pkneg, hm, sig, lines, count);
+        LAUNCH(k_rlc_accum_split<1>, ag.grid, ag.cta, s, n, g0, nc, (const fp*)lines, (const uint8_t*)bad, verdict, count);
+    }
+    LAUNCH(k_exact_publish, blocks_for(n, 256), 256, s, n, idx, (const uint8_t*)verdict, d_results, count);
+}
 // Message grouping of the device forms (device_forms.cuh): a hash table of >= 2k slots, the distinct messages' keys and points
 struct MsgGroups { uint32_t mask; uint32_t* slot_item; uint32_t* slot_rep; uint32_t* item_slot; uint32_t* pos; uint32_t* grp; uint8_t* keys;
                    unsigned* count; g2a* hm_d; uint8_t* ok_d; };
@@ -390,6 +417,95 @@ void launch_hash_grouped(cudaStream_t s, size_t k, const MsgGroups& m, const uin
     LAUNCH(k_broadcast_hm, blocks_for(k, 256), 256, s, k, (const uint32_t*)m.grp, (const g2a*)m.hm_d, (const uint8_t*)m.ok_d, hm, ok_hm);
 }
 #define STAGE_EV(i, sc, strm) do { if (g.stage_timing && (sc)->ev_ok) cudaEventRecord((sc)->ev[i], (strm)); } while (0)
+// the batched form (north-star "batched Miller loop + shared final exponentiation") of launch_verify_tail: strided groups of G rounds
+// (rlc_group_size), then the rounds of failed groups and the < G rounds that fill no group checked exactly; fills in bi
+template <int G> void launch_rlc_groups(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_t* ok_pk, uint8_t* d_results, cudaStream_t s,
+                                        hbls_batch_info& bi) {
+    const size_t ng = B / G, nr = ng * G, tail = B - nr;
+    const bool full = fills_chip(ng), two_phase = rlc_groups_two_phase(ng);
+    const Geom pg = pair_geom(2 * ng, full);                 // a lane pair per group
+    // blocks of HB_RLC_M groups: group g is member g / S of block g mod S; coefficients per (position, member)
+    const bool blocks = rlc_blocks(ng, two_phase);
+    const size_t S = blocks ? (((ng + HB_RLC_M - 1) / HB_RLC_M + 31) & ~(size_t)31) : 0;
+    // blocks possible: the device picks the form from how the last such call ended (k_rlc_form); counts[2] / counts[3] gate the
+    // group form's / block form's kernels, the scaling kernels take the matching coefficients
+    const unsigned* blk_gate = blocks ? v.counts + 3 : nullptr;
+    bool joint = false;
+    // the scaling stage with coefficients co / cb: drawn on the host (by value), or those k_rlc_draw wrote for this replay of a
+    // captured call (device pointers)
+    auto scale = [&](auto co, auto cb) {
+        if (blocks) LAUNCH(k_rlc_form, 1, 32, s, ng, g.rlc_block == 1 ? 1 : 0, (const int*)g.rlc_form, v.counts + 2);
+        if (g.scale_split && HB_BATCH_INV) {
+            LAUNCH(k_rlc_scale_g1, capped_blocks(nr, g.tpsm_scale_g1, TPB), TPB, s, nr, ng, v.apk, co, v.pk_scaled, S, cb, blk_gate);
+            const unsigned t = lockstep_cta(g.tpsm_scale_g2);
+            // the joint ladder runs a lane pair per GROUP: G times fewer items than the per-round ladder, so it needs a full chip of groups
+            joint = g.scale_joint >= 2 || (g.scale_joint == 1 && full);
+            if (joint) {          // one ladder per group into the Jacobian Sg (the first ng entries of S), then the shared-inversion affine form
+                LAUNCH(k_rlc_group_scale_g2_pair<G>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+                LAUNCH(k_g2_normalize_batch, heavy_blocks(ng), TPB, s, ng, (const g2*)v.S, v.Sg);
+            } else
+                LAUNCH(k_rlc_scale_g2_pair, capped_blocks(2 * nr, t, t), t, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
+        } else
+        LAUNCH(k_rlc_scale, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, (const uint64_t*)nullptr, v.pk_scaled, v.S, v.bad, S, cb, blk_gate);
+    };
+    if (g.cap_draw) scale(rlc_coeffs_dev{g.cap_draw->co.c}, rlc_block_coeffs_dev{g.cap_draw->cb.c});
+    else {
+        const rlc_coeffs co = rlc_draw();
+        const rlc_block_coeffs cb = blocks ? rlc_draw_block() : rlc_block_coeffs{};
+        scale(co, cb);
+    }
+    if (!joint) LAUNCH(k_rlc_group_sum<G>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
+    STAGE_EV(5, sc, s);
+    if (two_phase) {
+        // running points in their own kernel (lines to HBM, read once), accumulator + final exponentiation in the second.  Blocks
+        // possible (one chunk): both forms are launched and the device gates (k_rlc_form) let exactly one of them run.
+        const unsigned* gate_groups = blocks ? v.counts + 2 : nullptr;
+        const unsigned* gate_blocks = v.counts + 3;
+        const unsigned lt = lockstep_cta(g.tpsm_lines), at = lockstep_cta(g.tpsm_accum);
+        for (size_t g0 = 0; g0 < ng; g0 += rlc_chunk_groups()) {
+            const size_t ngc = ng - g0 < rlc_chunk_groups() ? ng - g0 : rlc_chunk_groups();
+            // the line kernel has G + 1 times the lane pairs
+            const Geom lg = pair_geom(2 * (G + 1) * ngc, full, lt, lt), ag = pair_geom(2 * ngc, full, at, at);
+            LAUNCH(k_rlc_lines_split<G>, lg.grid, lg.cta, s, ng, g0, ngc, v.pk_scaled, v.hm, v.Sg, v.lines, gate_groups);
+            if (blocks) LAUNCH(k_rlc_lines_blk<G>, lg.grid, lg.cta, s, ng, g0, ngc, v.pk_scaled, v.hm, v.lines, gate_blocks);
+            if (g0 == 0) { STAGE_EV(7, sc, s); sc->ev7_set = g.stage_timing && sc->ev_ok; }       // line kernel | accumulator kernel (first chunk)
+            LAUNCH(k_rlc_accum_split<G>, ag.grid, ag.cta, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, gate_groups);
+            if (blocks) LAUNCH(k_rlc_accum_blk<G>, ag.grid, ag.cta, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, v.fm, gate_blocks);
+        }
+        if (blocks) {
+            // one final exponentiation and one generator pair per block (warp per block), then the groups of the failed blocks
+            // alone: FE( their Miller value * Miller(B, Sg) ) == 1, a lane pair each, the list spread evenly over the lock-stepped
+            // CTAs.  group_ok then holds every group's own verdict, as without blocks.
+            LAUNCH(k_rlc_block_sum, heavy_blocks(S), TPB, s, S, ng, (const g2a*)v.Sg, v.Sb, gate_blocks);
+            LAUNCH(k_rlc_block_coop, coop_blocks(S), 32, s, S, ng, (const fp2*)v.fm, (const g2a*)v.Sb, (const uint8_t*)v.group_ok, v.block_ok, gate_blocks);
+            LAUNCH(k_rlc_block_list, blocks_for(ng, 256), 256, s, ng, S, (const uint8_t*)v.block_ok, v.group_ok, v.fail_list, v.counts + 4, gate_blocks);
+            LAUNCH(k_rlc_group_check_list, pg.grid, pg.cta, s, (const unsigned*)v.counts + 4, (const uint32_t*)v.fail_list, (const fp2*)v.fm,
+                   (const g2a*)v.Sg, v.group_ok);
+        }
+    } else
+        LAUNCH_SMEM(k_rlc_pairing_split<G>, pg.grid, pg.cta, HB_SMEM_F ? pg.cta * HB_SMEM_F_WORDS * 4 : 0, s, ng, v.pk_scaled, v.hm, v.Sg, v.bad, v.group_ok);
+    // exact pass over the rounds of failed groups only (compacted on the device; the launches are sized for the worst case and
+    // return at once when the list is short or empty)
+    LAUNCH(k_rlc_finish, blocks_for(nr, 256), 256, s, nr, ng, v.group_ok, d_results, v.fail_list, v.counts);
+    if (blocks) LAUNCH(k_rlc_form_update, 1, 32, s, ng, (const unsigned*)v.counts, g.rlc_form);     // the next call's form
+    LAUNCH(k_g1_normalize_list, heavy_blocks(nr), TPB, s, v.counts, v.fail_list, v.apk, v.pkneg, 1);
+    if (two_phase && g.exact_two_phase)          // gathered into pk_scaled and S, both free after the group pass
+        launch_exact_two_phase(nr, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, v.bad, v.verdict, v.ex_lines, d_results, s, v.fail_list, v.counts,
+                               v.pk_scaled, v.ex_hm, reinterpret_cast<g2a*>(v.S));
+    else {
+        const Geom lg = pair_geom(2 * nr, fills_chip(nr));
+        LAUNCH(k_pairing_verify_split_list, lg.grid, lg.cta, s, v.counts, v.fail_list, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results);
+    }
+    LAUNCH(k_pairing_fixup_list, heavy_blocks(nr), TPB, s, v.counts, v.fail_list, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results);
+    if (tail) {       // the < G rounds that do not fill a group are always verified exactly
+        LAUNCH(k_g1_normalize, 1, TPB, s, tail, v.apk + nr, v.pkneg + nr, 1, (const int*)nullptr);
+        LAUNCH(k_pairing_verify_split, blocks_for(2 * tail, 64), 64, s, tail, v.sig + nr, v.pkneg + nr, v.hm + nr, v.ok_sig + nr, v.ok_hm + nr,
+               ok_pk ? ok_pk + nr : (const uint8_t*)nullptr, d_results + nr, (const int*)nullptr);
+        LAUNCH(k_pairing_fixup, 1, TPB, s, tail, v.sig + nr, v.pkneg + nr, v.hm + nr, v.ok_sig + nr, v.ok_hm + nr,
+               ok_pk ? ok_pk + nr : (const uint8_t*)nullptr, d_results + nr, (const int*)nullptr);
+    }
+    bi.group_size = (int32_t)G; bi.groups = ng; bi.tail_rounds = (uint32_t)tail; bi.cta_threads = pg.cta;
+}
 // v.apk holds the Jacobian (aggregate) public key of every round; ok_pk (nullable) = per-round "key decoded" flags of the triple form
 // h_msg (nullable): host copy of THE message when the call has a single one (one round, or a same-message batch) -- the key of the
 // H(m) cache.  mg (nullable, device forms): H(m) once per distinct message, grouped on the device (same_msg / h_msg unused)
@@ -409,8 +525,7 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
     const bool forked = pairs && sc->forked;              // decode on aux[0], hash on aux[1], concurrently with the work above
     cudaStream_t sd = forked ? g.aux[0] : s, sh = forked ? g.aux[1] : s;
     if (forked) { cudaStreamWaitEvent(sd, sc->fork, 0); cudaStreamWaitEvent(sh, sc->fork, 0); }
-    const size_t coop_cap = (size_t)g.sm_count * (size_t)(g.coop_wpsm > 0 ? g.coop_wpsm : 1);      // resident warps (one round each)
-    const unsigned coop_grid = (unsigned)(B < coop_cap ? B : coop_cap);
+    const unsigned coop_grid = coop_blocks(B);
     const bool split_ml = forked && v.f1 != nullptr;       // Miller value of (B, sigma) on the decode stream, beside hash-to-G2
     // one message (one round, or a same-message batch): H(m) once -- from the cache when this node has hashed it before (it signed
     // it, verified it, or prefetched it)
@@ -458,128 +573,12 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
     hbls_batch_info& bi = g.cap_draw ? cap_info : g.info;
     bi = hbls_batch_info{}; bi.rounds = B; bi.mode = rlc ? 1 : 0;
     cudaMemsetAsync(v.counts, 0, 5 * sizeof(unsigned), s);
-    if (rlc) {
-        // batched form (north-star "batched Miller loop + shared final exponentiation"): strided groups of G rounds; G = 8 once
-        // that still gives every SM a full CTA of lane pairs (fewer Miller-loop pairs and final exponentiations per round), else 4
-        const size_t G = rlc_group_size(B);
-        const size_t ng = B / G, nr = ng * G, tail = B - nr;
-        const bool full = 2 * ng >= (size_t)g.sm_count * HB_TPB_SPLIT;
-        const unsigned pb = full ? split_blocks(2 * ng) : blocks_for(2 * ng, 64), pt = full ? HB_TPB_SPLIT : 64;
-        const bool two_phase = g.rlc_two_phase && v.lines != nullptr && (full || g.rlc_two_phase >= 2);
-        // blocks of HB_RLC_M groups: group g is member g / S of block g mod S; coefficients per (position, member)
-        const bool blocks = rlc_blocks(ng, two_phase);
-        const size_t S = blocks ? (((ng + HB_RLC_M - 1) / HB_RLC_M + 31) & ~(size_t)31) : 0;
-        // blocks possible: the device picks the form from how the last such call ended (k_rlc_form); counts[2] / counts[3] gate the
-        // group form's / block form's kernels, the scaling kernels take the matching coefficients
-        const unsigned* blk_gate = blocks ? v.counts + 3 : nullptr;
-        bool joint = false;
-        // the scaling stage with coefficients co / cb: drawn on the host (by value), or those k_rlc_draw wrote for this replay of a
-        // captured call (device pointers)
-        auto scale = [&](auto co, auto cb) {
-            if (blocks) LAUNCH(k_rlc_form, 1, 32, s, ng, g.rlc_block == 1 ? 1 : 0, (const int*)g.rlc_form, v.counts + 2);
-            if (g.scale_split && HB_BATCH_INV) {
-                LAUNCH(k_rlc_scale_g1, capped_blocks(nr, g.tpsm_scale_g1, TPB), TPB, s, nr, ng, v.apk, co, v.pk_scaled, S, cb, blk_gate);
-                const unsigned t = lockstep_cta(g.tpsm_scale_g2);
-                // the joint ladder runs a lane pair per GROUP: G times fewer items than the per-round ladder, so it needs a full chip of groups
-                joint = g.scale_joint >= 2 || (g.scale_joint == 1 && full);
-                if (joint) {          // one ladder per group into the Jacobian Sg (the first ng entries of S), then the shared-inversion affine form
-                    if (G == 8) LAUNCH(k_rlc_group_scale_g2_pair<8>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
-                    else LAUNCH(k_rlc_group_scale_g2_pair<4>, capped_blocks(2 * ng, t, t), t, s, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
-                    LAUNCH(k_g2_normalize_batch, heavy_blocks(ng), TPB, s, ng, (const g2*)v.S, v.Sg);
-                } else
-                    LAUNCH(k_rlc_scale_g2_pair, capped_blocks(2 * nr, t, t), t, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, v.S, v.bad, S, cb, blk_gate);
-            } else
-            LAUNCH(k_rlc_scale, capped_blocks(nr, g.tpsm_scale, TPB), TPB, s, nr, ng, v.apk, v.sig, v.hm, v.ok_sig, v.ok_hm, ok_pk, co, (const uint64_t*)nullptr, v.pk_scaled, v.S, v.bad, S, cb, blk_gate);
-        };
-        if (g.cap_draw) scale(rlc_coeffs_dev{g.cap_draw->co.c}, rlc_block_coeffs_dev{g.cap_draw->cb.c});
-        else {
-            const rlc_coeffs co = rlc_draw();
-            const rlc_block_coeffs cb = blocks ? rlc_draw_block() : rlc_block_coeffs{};
-            scale(co, cb);
-        }
-        if (!joint && G == 8) LAUNCH(k_rlc_group_sum<8>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
-        else if (!joint) LAUNCH(k_rlc_group_sum<4>, heavy_blocks(ng), TPB, s, ng, v.S, v.Sg);
-        STAGE_EV(5, sc, s);
-        if (two_phase) {
-            // running points in their own kernel (lines to HBM, read once), accumulator + final exponentiation in the second
-            for (size_t g0 = 0; g0 < ng; g0 += rlc_chunk_groups()) {
-                const size_t ngc = ng - g0 < rlc_chunk_groups() ? ng - g0 : rlc_chunk_groups();
-                // a batch that does not fill the chip: 64-thread CTAs spread over the SMs (the line kernel has G + 1 times the lane pairs)
-                const unsigned lt = full ? lockstep_cta(g.tpsm_lines) : 64, at = full ? lockstep_cta(g.tpsm_accum) : 64;
-                const unsigned lb = full ? capped_blocks(2 * (G + 1) * ngc, lt, lt) : blocks_for(2 * (G + 1) * ngc, 64);
-                const unsigned ab = full ? capped_blocks(2 * ngc, at, at) : blocks_for(2 * ngc, 64);
-                // blocks possible (one chunk): both forms are launched and the device gates (k_rlc_form) let exactly one of them run
-                const unsigned* gate_groups = blocks ? v.counts + 2 : nullptr;
-                const unsigned* gate_blocks = v.counts + 3;
-                if (G == 8) LAUNCH(k_rlc_lines_split<8>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.Sg, v.lines, gate_groups);
-                else LAUNCH(k_rlc_lines_split<4>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.Sg, v.lines, gate_groups);
-                if (blocks && G == 8) LAUNCH(k_rlc_lines_blk<8>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.lines, gate_blocks);
-                else if (blocks) LAUNCH(k_rlc_lines_blk<4>, lb, lt, s, ng, g0, ngc, v.pk_scaled, v.hm, v.lines, gate_blocks);
-                if (g0 == 0) { STAGE_EV(7, sc, s); sc->ev7_set = g.stage_timing && sc->ev_ok; }       // line kernel | accumulator kernel (first chunk)
-                if (G == 8) LAUNCH(k_rlc_accum_split<8>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, gate_groups);
-                else LAUNCH(k_rlc_accum_split<4>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, gate_groups);
-                if (blocks && G == 8) LAUNCH(k_rlc_accum_blk<8>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, rlc_fm(v, G, ng), gate_blocks);
-                else if (blocks) LAUNCH(k_rlc_accum_blk<4>, ab, at, s, ng, g0, ngc, (const fp*)v.lines, v.bad, v.group_ok, rlc_fm(v, G, ng), gate_blocks);
-            }
-            if (blocks) {
-                // one final exponentiation and one generator pair per block (warp per block), then the groups of the failed blocks
-                // alone: FE( their Miller value * Miller(B, Sg) ) == 1, a lane pair each, the list spread evenly over the lock-stepped
-                // CTAs.  group_ok then holds every group's own verdict, as without blocks.
-                fp2* fm = rlc_fm(v, G, ng);
-                const unsigned cb_grid = full ? split_blocks(2 * ng) : blocks_for(2 * ng, 64), cb_tpb = full ? HB_TPB_SPLIT : 64;
-                const unsigned* gate = v.counts + 3;
-                LAUNCH(k_rlc_block_sum, heavy_blocks(S), TPB, s, S, ng, (const g2a*)v.Sg, v.Sb, gate);
-                const size_t coop_cap = (size_t)g.sm_count * (size_t)(g.coop_wpsm > 0 ? g.coop_wpsm : 1);
-                LAUNCH(k_rlc_block_coop, (unsigned)(S < coop_cap ? S : coop_cap), 32, s, S, ng, (const fp2*)fm, (const g2a*)v.Sb, (const uint8_t*)v.group_ok, v.block_ok, gate);
-                LAUNCH(k_rlc_block_list, blocks_for(ng, 256), 256, s, ng, S, (const uint8_t*)v.block_ok, v.group_ok, v.fail_list, v.counts + 4, gate);
-                LAUNCH(k_rlc_group_check_list, cb_grid, cb_tpb, s, (const unsigned*)v.counts + 4, (const uint32_t*)v.fail_list, (const fp2*)fm,
-                       (const g2a*)v.Sg, v.group_ok);
-            }
-        } else if (G == 8)
-            LAUNCH_SMEM(k_rlc_pairing_split<8>, pb, pt, HB_SMEM_F ? pt * HB_SMEM_F_WORDS * 4 : 0, s, ng, v.pk_scaled, v.hm, v.Sg, v.bad, v.group_ok);
-        else
-            LAUNCH_SMEM(k_rlc_pairing_split<4>, pb, pt, HB_SMEM_F ? pt * HB_SMEM_F_WORDS * 4 : 0, s, ng, v.pk_scaled, v.hm, v.Sg, v.bad, v.group_ok);
-        // exact pass over the rounds of failed groups only (compacted on the device; the launches are sized for the worst case and
-        // return at once when the list is short or empty)
-        LAUNCH(k_rlc_finish, blocks_for(nr, 256), 256, s, nr, ng, v.group_ok, d_results, v.fail_list, v.counts);
-        if (blocks) LAUNCH(k_rlc_form_update, 1, 32, s, ng, (const unsigned*)v.counts, g.rlc_form);     // the next call's form
-        LAUNCH(k_g1_normalize_list, heavy_blocks(nr), TPB, s, v.counts, v.fail_list, v.apk, v.pkneg, 1);
-        if (two_phase && g.exact_two_phase) {
-            // the listed rounds, gathered into contiguous arrays, through the line / accumulator kernels as "groups" of one round; the
-            // launches are sized for the worst case and return at once beyond the device-side count
-            const size_t nlc = nr < rlc_chunk_groups() ? nr : rlc_chunk_groups();
-            g2a* hm_c = reinterpret_cast<g2a*>(v.lines + (size_t)HB_ML_STEPS * 3 * 2 * nlc * 2);      // behind the chunk's lines
-            g2a* sig_c = reinterpret_cast<g2a*>(v.S); g1a* pk_c = v.pk_scaled;                        // both free after the group pass
-            const unsigned* cnt = v.counts;
-            LAUNCH(k_exact_prepare, blocks_for(nr, 256), 256, s, nr, (const uint32_t*)v.fail_list, (const g2a*)v.sig, (const g1a*)v.pkneg, (const g2a*)v.hm,
-                   (const uint8_t*)v.ok_sig, (const uint8_t*)v.ok_hm, ok_pk, pk_c, hm_c, sig_c, v.bad, d_results, cnt);
-            const bool lfull = 2 * nr >= (size_t)g.sm_count * HB_TPB_SPLIT;
-            const unsigned bt = lfull ? HB_TPB_SPLIT : 64;
-            for (size_t g0 = 0; g0 < nr; g0 += rlc_chunk_groups()) {
-                const size_t nc = nr - g0 < rlc_chunk_groups() ? nr - g0 : rlc_chunk_groups();
-                const unsigned lb = lfull ? split_blocks(4 * nc) : blocks_for(4 * nc, 64), ab = lfull ? split_blocks(2 * nc) : blocks_for(2 * nc, 64);
-                LAUNCH(k_rlc_lines_split<1>, lb, bt, s, nr, g0, nc, (const g1a*)pk_c, (const g2a*)hm_c, (const g2a*)sig_c, v.lines, cnt);
-                LAUNCH(k_rlc_accum_split<1>, ab, bt, s, nr, g0, nc, (const fp*)v.lines, (const uint8_t*)v.bad, v.verdict, cnt);
-            }
-            LAUNCH(k_exact_publish, blocks_for(nr, 256), 256, s, nr, (const uint32_t*)v.fail_list, (const uint8_t*)v.verdict, d_results, cnt);
-        } else if (2 * nr >= (size_t)g.sm_count * HB_TPB_SPLIT)
-            LAUNCH(k_pairing_verify_split_list, split_blocks(2 * nr), HB_TPB_SPLIT, s, v.counts, v.fail_list, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results);
-        else
-            LAUNCH(k_pairing_verify_split_list, blocks_for(2 * nr, 64), 64, s, v.counts, v.fail_list, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results);
-        LAUNCH(k_pairing_fixup_list, heavy_blocks(nr), TPB, s, v.counts, v.fail_list, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results);
-        if (tail) {       // the < G rounds that do not fill a group are always verified exactly
-            LAUNCH(k_g1_normalize, 1, TPB, s, tail, v.apk + nr, v.pkneg + nr, 1, (const int*)nullptr);
-            LAUNCH(k_pairing_verify_split, blocks_for(2 * tail, 64), 64, s, tail, v.sig + nr, v.pkneg + nr, v.hm + nr, v.ok_sig + nr, v.ok_hm + nr,
-                   ok_pk ? ok_pk + nr : (const uint8_t*)nullptr, d_results + nr, (const int*)nullptr);
-            LAUNCH(k_pairing_fixup, 1, TPB, s, tail, v.sig + nr, v.pkneg + nr, v.hm + nr, v.ok_sig + nr, v.ok_hm + nr,
-                   ok_pk ? ok_pk + nr : (const uint8_t*)nullptr, d_results + nr, (const int*)nullptr);
-        }
-        bi.group_size = (int32_t)G; bi.groups = ng; bi.tail_rounds = (uint32_t)tail; bi.cta_threads = pt;
-    } else {
+    if (rlc) (rlc_group_size(B) == 8 ? launch_rlc_groups<8> : launch_rlc_groups<4>)(B, v, sc, ok_pk, d_results, s, bi);
+    else {
         // exact form at every batch size: a lane pair per round.  Large batches use 512-thread lock-stepped CTAs (one per SM),
         // small ones 64-thread CTAs spread over the SMs.
         STAGE_EV(5, sc, s);
-        const bool full = 2 * B >= (size_t)g.sm_count * HB_TPB_SPLIT;
+        const Geom pg = pair_geom(2 * B, fills_chip(B));
         const bool coop = (long long)B <= g.coop_max;        // latency form: one warp per round (vm.cuh), up to 14 resident rounds per SM (15 KB of slots each)
         if (coop && warm)
             LAUNCH(k_fe2_coop, coop_grid, 32, s, B, v.f1, v.irr1, v.f2, v.irr2, v.ok_sig, v.ok_hm, ok_pk, (const uint8_t*)nullptr, d_results);
@@ -587,14 +586,12 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
             LAUNCH(k_pairing_coop2, coop_grid, 32, s, B, v.f1, v.irr1, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results);
         else if (coop)
             LAUNCH(k_pairing_coop, coop_grid, 32, s, B, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results);
-        else if (exact_two_phase(B) && v.lines)
-            launch_exact_two_phase(B, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, v.bad, v.verdict, v.lines, d_results, s);
-        else if (full)
-            LAUNCH(k_pairing_verify_split, split_blocks(2 * B), HB_TPB_SPLIT, s, B, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results, (const int*)nullptr);
+        else if (exact_two_phase(B))
+            launch_exact_two_phase(B, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, v.bad, v.verdict, v.ex_lines, d_results, s);
         else
-            LAUNCH(k_pairing_verify_split, blocks_for(2 * B, 64), 64, s, B, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results, (const int*)nullptr);
+            LAUNCH(k_pairing_verify_split, pg.grid, pg.cta, s, B, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results, (const int*)nullptr);
         LAUNCH(k_pairing_fixup, heavy_blocks(B), TPB, s, B, v.sig, v.pkneg, v.hm, v.ok_sig, v.ok_hm, ok_pk, d_results, (const int*)nullptr);
-        bi.cta_threads = coop ? 32 : (full ? HB_TPB_SPLIT : 64);
+        bi.cta_threads = coop ? 32 : pg.cta;
     }
     STAGE_EV(6, sc, s);
     if (g.cap_draw) return;                                    // captured: no host copy, no event, no batch info
@@ -602,21 +599,6 @@ void launch_verify_tail(size_t B, const VerifyBufs& v, Scratch* sc, const uint8_
     cudaEventRecord(sc->done, s);
     g.info_sc = sc; g.info_valid = true;
     if (g.stage_timing && sc->ev_ok) g.stage_sc = sc;
-}
-
-void launch_exact_two_phase(size_t n, const g2a* sig, const g1a* pkneg, const g2a* hm, const uint8_t* ok_a, const uint8_t* ok_b, const uint8_t* ok_c,
-                            uint8_t* bad, uint8_t* verdict, fp* lines, uint8_t* d_results, cudaStream_t s) {
-    LAUNCH(k_exact_prepare, blocks_for(n, 256), 256, s, n, (const uint32_t*)nullptr, sig, pkneg, hm, ok_a, ok_b, ok_c,
-           (g1a*)nullptr, (g2a*)nullptr, (g2a*)nullptr, bad, d_results);
-    const bool full = 2 * n >= (size_t)g.sm_count * HB_TPB_SPLIT;
-    for (size_t g0 = 0; g0 < n; g0 += rlc_chunk_groups()) {
-        const size_t nc = n - g0 < rlc_chunk_groups() ? n - g0 : rlc_chunk_groups();
-        const unsigned bt = full ? HB_TPB_SPLIT : 64;
-        const unsigned lb = full ? split_blocks(4 * nc) : blocks_for(4 * nc, 64), ab = full ? split_blocks(2 * nc) : blocks_for(2 * nc, 64);
-        LAUNCH(k_rlc_lines_split<1>, lb, bt, s, n, g0, nc, pkneg, hm, sig, lines);
-        LAUNCH(k_rlc_accum_split<1>, ab, bt, s, n, g0, nc, (const fp*)lines, (const uint8_t*)bad, verdict);
-    }
-    LAUNCH(k_exact_publish, blocks_for(n, 256), 256, s, n, (const uint32_t*)nullptr, (const uint8_t*)verdict, d_results);
 }
 
 // secret-key bytes on the host (secret_key.hpp): base-Z digits, the range check and equality in constant time, and wiping
@@ -793,8 +775,7 @@ int part1_locked(Part1Req* const* rq, size_t n, const g1* d_apk = nullptr, const
     if (gather) LAUNCH(k_broadcast_hm, blocks_for(nh, 256), 256, s, nh, (const uint32_t*)(din + i_idx), (const g2a*)th, (const uint8_t*)tok, hm, ok_hm);
     if (nv) {
         uint8_t* dres = dout + o_res;
-        const size_t coop_cap = (size_t)g.sm_count * (size_t)(g.coop_wpsm > 0 ? g.coop_wpsm : 1);
-        if (g.coop_max >= 1) LAUNCH(k_pairing_coop, (unsigned)(nv < coop_cap ? nv : coop_cap), 32, s, nv, vsig, pkneg, hm, (const uint8_t*)ok_hm, vok_sig, (const uint8_t*)nullptr, dres);
+        if (g.coop_max >= 1) LAUNCH(k_pairing_coop, coop_blocks(nv), 32, s, nv, vsig, pkneg, hm, (const uint8_t*)ok_hm, vok_sig, (const uint8_t*)nullptr, dres);
         else LAUNCH(k_pairing_verify_split, blocks_for(2 * nv, 64), 64, s, nv, vsig, pkneg, hm, (const uint8_t*)ok_hm, vok_sig, (const uint8_t*)nullptr, dres, (const int*)nullptr);
         LAUNCH(k_pairing_fixup, blocks_for(nv, 32), 32, s, nv, vsig, pkneg, hm, (const uint8_t*)ok_hm, vok_sig, (const uint8_t*)nullptr, dres, (const int*)nullptr);
     }

@@ -81,7 +81,7 @@ template <int G> static int block_verify(uint32_t n, const uint8_t* pks48, size_
     std::vector<g2a> Sg(ng + 1), Sb(S); std::vector<uint8_t> group_ok(ng + 1, 0xee), block_ok(S, 0xee);
     run_seq(1, 2, [&] { k_rlc_group_sum<G>(ng, Sj.data(), Sg.data()); });
     std::vector<fp> lines((size_t)HB_ML_STEPS * 3 * (G + 1) * ng * 2);
-    fp2* fm = reinterpret_cast<fp2*>(lines.data() + (size_t)HB_ML_STEPS * 3 * G * ng * 2);       // hbls.cu rlc_fm
+    fp2* fm = reinterpret_cast<fp2*>(lines.data() + (size_t)HB_ML_STEPS * 3 * G * ng * 2);       // the groups' Miller values (hbls.cu: VerifyBufs::fm)
     const unsigned* nocount = nullptr;
     run_pair([&] { k_rlc_lines_blk<G>(ng, 0, ng, pk_scaled.data(), hm.data(), lines.data(), nocount); });
     run_pair([&] { k_rlc_accum_blk<G>(ng, 0, ng, lines.data(), bad.data(), group_ok.data(), fm, nocount); });
