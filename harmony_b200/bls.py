@@ -110,6 +110,10 @@ def lib():
         sig("hbls_verify_batch_status_device", c.c_int, sz, vp, vp, vp, sz, vp, vp)
         sig("hbls_verify_headers_device", c.c_int, vp, sz, vp, vp, sz, vp, sz, sz, vp, vp)
         sig("hbls_aggregate_verify_items_device", c.c_int, sz, c.POINTER(vp), vp, vp, vp, sz, vp, vp)
+        sig("hbls_committee_set_create", c.c_int, c.POINTER(vp), c.POINTER(vp), sz)
+        sig("hbls_committee_set_destroy", None, vp)
+        sig("hbls_committee_set_size", sz, vp)
+        sig("hbls_aggregate_verify_set_device", c.c_int, vp, sz, vp, vp, vp, vp, sz, vp, vp)
         sig("hbls_rlc_partial", c.c_int, sz, vp, vp, vp, sz, vp)
         sig("hbls_rlc_fold", c.c_int, sz, vp)
         sig("hbls_mask_create", c.c_int, c.POINTER(vp), vp)
@@ -495,6 +499,50 @@ def AggregateVerifyItemsDevice(committees, bitmaps, sigs, msgs, stream=None):
         raise HblsError("hbls_aggregate_verify_items_device cannot be captured into a CUDA graph (HBLS_ERR_CAPTURE): nothing was enqueued")
     if rc != 0: raise HblsError(f"hbls_aggregate_verify_items_device rc={rc}")
     return out
+
+# hbls_aggregate_verify_set_device: the result of an item whose committee index is not in the set (include/hbls.h)
+SET_BAD_INDEX = 48
+
+class CommitteeSet:
+    """hbls_committee_set: m committees registered once, their descriptors in HBM, so that the items of a multi-committee batch
+    can name their committee by an index tensor on the device (one set per shard / epoch table, as the reference keeps one epochCtx
+    each).  Keeps the Committee objects alive for as long as the set lives."""
+    def __init__(self, committees):
+        L = _need()
+        self.committees = list(committees)
+        m = len(self.committees)
+        if m == 0 or m > 2 ** 31: raise ValueError(f"a committee set holds 1 .. 2^31 committees, got {m}")   # int32 indices: negative is never one
+        arr = (ctypes.c_void_p * m)(*[c.h for c in self.committees])
+        self.h = ctypes.c_void_p()
+        rc = L.hbls_committee_set_create(ctypes.byref(self.h), arr, m)
+        if rc != 0: raise HblsError(f"hbls_committee_set_create rc={rc}")
+    def __del__(self):
+        try:
+            if self.h and _lib is not None: _lib.hbls_committee_set_destroy(self.h); self.h = None
+        except Exception: pass
+    def __len__(self): return len(self.committees)
+
+    def AggregateVerifyDevice(self, index, bitmaps, sigs, msgs, stream=None):
+        """hbls_aggregate_verify_set_device: item j = (committee index[j] of the set, its bitmap, sigs[j], msgs[j]) -> uint8 tensor
+        [k] of 1 / 0, or SET_BAD_INDEX where index[j] is negative or >= len(self), filled asynchronously on `stream` (default:
+        torch.cuda.current_stream()); capturable with torch.cuda.graph.  index: int32 CUDA tensor [k].  bitmaps: the items' bitmaps
+        back to back (an item with a bad index has none), 1-D, or [k, blen] when every item's committee has blen bitmap bytes; the
+        indices live on the device, so their total is not checked here: the caller supplies the bytes they name."""
+        import torch
+        L = _need()
+        k = _rows(sigs, "sigs", 96)
+        msg_len = _rows_any(msgs, "msgs", k)
+        if not isinstance(index, torch.Tensor) or index.dtype != torch.int32 or index.dim() != 1 or index.numel() != k:
+            raise HblsError(f"index: expected a 1-D torch.int32 tensor of {k} values")
+        if index.device != sigs.device or not index.is_contiguous(): raise HblsError(f"index: on {index.device}, expected {sigs.device}, contiguous")
+        _check_tensor(bitmaps, "bitmaps")
+        if bitmaps.dim() not in (1, 2) or (bitmaps.dim() == 2 and bitmaps.shape[0] != k):
+            raise HblsError(f"bitmaps: shape {tuple(bitmaps.shape)}, expected the items' bitmaps back to back ([k, blen] or 1-D)")
+        st, out, h = _device_call(stream, k, (index, bitmaps, sigs, msgs))
+        if k == 0: return out
+        rc = L.hbls_aggregate_verify_set_device(self.h, k, _ptr(index), _ptr(bitmaps), _ptr(sigs), _ptr(msgs), msg_len, _ptr(out), h)
+        if rc != 0: raise HblsError(f"hbls_aggregate_verify_set_device rc={rc}")
+        return out
 
 PARTIAL_BYTES = 872
 def RlcPartial(pks48: bytes, sigs96: bytes, msgs: bytes, msg_len: int) -> bytes:

@@ -29,6 +29,13 @@ struct hbls_committee {
     g1* total = nullptr;        // device, sum of all rows (lets dense bitmaps be aggregated from their complement)
     ~hbls_committee() { if (table) cudaFree(table); if (total) cudaFree(total); }
 };
+// committee set: m committees registered once, their descriptors (key table, slots) in HBM, so that the items of a multi-committee
+// batch can name their committee by an index in device memory (hbls_aggregate_verify_set_device)
+struct hbls_committee_set {
+    size_t m = 0;
+    hb::set_entry* ents = nullptr;      // device
+    ~hbls_committee_set() { if (ents) cudaFree(ents); }
+};
 struct hbls_mask {
     const hbls_committee* c = nullptr;
     std::vector<uint8_t> bitmap;        // Mask.Bitmap (host)
@@ -1419,8 +1426,18 @@ static void verify_headers_body(const hbls_committee* c, size_t n, const uint8_t
     LAUNCH(k_pack_flags, blocks_for(n, 256), 256, s, n, v.ok_sig, v.ok_hm, (const uint8_t*)nullptr, v.flags);
     LAUNCH(k_status_headers, blocks_for(n, 256), 256, s, n, c->n, d_bitmaps, blen, quorum, (const uint8_t*)v.flags, (const uint8_t*)d_results, d_status);
 }
-// items of a multi-committee batch (their bitmaps back to back in d_bitmaps): verdicts into d_results, ditems = k descriptors (table,
-// bitmap, slots per item), which come from the host array of handles.  They are written into the stream's own pinned buffer and uploaded
+// items of a multi-committee batch (their bitmaps back to back in d_bitmaps) once their descriptors ditems (table, bitmap, slots per
+// item) are in HBM: each item's key summed from its committee's table, then the verify tail, verdicts into d_results.  ok_key
+// (nullable): the committee-set form's "index < m" flags, which the tail reads as "key decoded".
+static void verify_items_tail(size_t k, const mask_item* ditems, const uint8_t* ok_key, const uint8_t* d_sigs, const uint8_t* d_msgs,
+                              size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, const VerifyBufs& v, bool same_msg,
+                              const MsgGroups* mg) {
+    fork_point(k, sc, s);
+    STAGE_EV(0, sc, s);
+    LAUNCH(k_mask_aggregate_items, blocks_for(k * 32, 128), 128, s, k, ditems, v.apk);
+    launch_verify_tail(k, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, ok_key, d_results, s, same_msg, nullptr, mg);
+}
+// the host-array forms' descriptors, from the host array of handles.  They are written into the stream's own pinned buffer and uploaded
 // with an asynchronous copy; an event recorded after that copy guards the buffer, so a later call on the same stream waits (on the
 // host) only if the earlier upload has not run yet.  A pageable copy would synchronise the stream.
 static int verify_items_body(size_t k, const hbls_committee* const* committees, const uint8_t* d_bitmaps, const uint8_t* d_sigs,
@@ -1441,11 +1458,24 @@ static int verify_items_body(size_t k, const hbls_committee* const* committees, 
     }
     CK(cudaMemcpyAsync(ditems, sc->h_items, k * sizeof(mask_item), cudaMemcpyHostToDevice, s));
     CK(cudaEventRecord(sc->items_copied, s)); sc->items_pending = true;
-    fork_point(k, sc, s);
-    STAGE_EV(0, sc, s);
-    LAUNCH(k_mask_aggregate_items, blocks_for(k * 32, 128), 128, s, k, (const mask_item*)ditems, v.apk);
-    launch_verify_tail(k, v, sc, d_sigs, d_msgs, (uint32_t)msg_len, nullptr, d_results, s, same_msg, nullptr, mg);
+    verify_items_tail(k, ditems, nullptr, d_sigs, d_msgs, msg_len, d_results, s, sc, v, same_msg, mg);
     return 0;
+}
+// the committee-set form's descriptors, built on the device from d_index (kernels.cuh k_set_*): nothing is staged from the host, so
+// the call can be captured.  tile_sum: one entry per HB_SET_TILE items.  A bad index's result is HBLS_SET_BAD_INDEX, written after the
+// tail (which has read it as an undecodable key: no verdict of its own, no effect on its group).
+struct SetBufs { mask_item* items; uint64_t* tile_sum; };
+static SetBufs carve_set(Arena& ar, size_t k) { return SetBufs{ar.take<mask_item>(k), ar.take<uint64_t>((k + HB_SET_TILE - 1) / HB_SET_TILE)}; }
+static void verify_set_body(const hbls_committee_set* set, size_t k, const uint32_t* d_index, const uint8_t* d_bitmaps, const uint8_t* d_sigs,
+                            const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s, Scratch* sc, const SetBufs& b,
+                            const VerifyBufs& v, const MsgGroups& mg) {
+    const size_t nt = (k + HB_SET_TILE - 1) / HB_SET_TILE;
+    const uint32_t m = (uint32_t)set->m;
+    LAUNCH(k_set_tile_sums, (unsigned)nt, HB_SET_TILE, s, k, d_index, m, (const set_entry*)set->ents, b.tile_sum);
+    LAUNCH(k_set_tile_scan, 1, HB_SET_TILE, s, nt, b.tile_sum);
+    LAUNCH(k_set_items, (unsigned)nt, HB_SET_TILE, s, k, d_index, m, (const set_entry*)set->ents, (const uint64_t*)b.tile_sum, d_bitmaps, b.items, v.ok_pk);
+    verify_items_tail(k, b.items, v.ok_pk, d_sigs, d_msgs, msg_len, d_results, s, sc, v, false, &mg);
+    LAUNCH(k_set_bad_index, blocks_for(k, 256), 256, s, k, (const uint8_t*)v.ok_pk, d_results);
 }
 
 // ------------------------------------------------------------------ host forms: the inputs staged on g.stream, one synchronise
@@ -1614,6 +1644,46 @@ int hbls_aggregate_verify_items_device(size_t k, const hbls_committee* const* co
     if (cap) return cap < 0 ? cap : HBLS_ERR_CAPTURE;
     return aggregate_verify_items_device_locked(k, committees, (const uint8_t*)d_bitmaps, (const uint8_t*)d_sigs96, (const uint8_t*)d_msgs, msg_len,
                                                 (uint8_t*)d_results, s);
+}
+
+// ------------------------------------------------------------------ committee sets
+static_assert(HB_SET_BAD_INDEX == HBLS_SET_BAD_INDEX, "status codes");
+static int committee_set_create_locked(hbls_committee_set** out, const hbls_committee* const* committees, size_t m) {
+    std::vector<set_entry> ents(m);
+    for (size_t i = 0; i < m; i++) ents[i] = set_entry{committees[i]->table, (uint64_t)committees[i]->n};
+    std::unique_ptr<hbls_committee_set> set(new hbls_committee_set);
+    set->m = m;
+    CK(cudaMalloc(&set->ents, m * sizeof(set_entry)));
+    CK(cudaMemcpy(set->ents, ents.data(), m * sizeof(set_entry), cudaMemcpyHostToDevice));
+    *out = set.release();
+    return 0;
+}
+int hbls_committee_set_create(hbls_committee_set** out, const hbls_committee* const* committees, size_t m) {
+    if (int e = ensure_init()) return e;
+    if (!out || !committees || m == 0 || m > UINT32_MAX) return HBLS_ERR_ARG;
+    for (size_t i = 0; i < m; i++) if (!committees[i]) return HBLS_ERR_ARG;
+    HostLock lk;
+    return committee_set_create_locked(out, committees, m);
+}
+void hbls_committee_set_destroy(hbls_committee_set* s) { if (!s) return; HostLock lk; cudaDeviceSynchronize(); delete s; }
+size_t hbls_committee_set_size(const hbls_committee_set* s) { return s ? s->m : 0; }
+static int aggregate_verify_set_device_locked(const hbls_committee_set* set, size_t k, const uint32_t* d_index, const uint8_t* d_bitmaps,
+                                              const uint8_t* d_sigs, const uint8_t* d_msgs, size_t msg_len, uint8_t* d_results, cudaStream_t s) {
+    return run_device_form(s, k, [&](Arena& ar) { return std::tuple{carve_groups(ar, k), carve_verify(ar, k), carve_set(ar, k)}; },
+                           [&](Scratch* sc, const auto& bufs) {
+        const auto& [mg, v, b] = bufs;
+        verify_set_body(set, k, d_index, d_bitmaps, d_sigs, d_msgs, msg_len, d_results, s, sc, b, v, mg);
+    });
+}
+int hbls_aggregate_verify_set_device(const hbls_committee_set* set, size_t k, const void* d_index, const void* d_bitmaps, const void* d_sigs96,
+                                     const void* d_msgs, size_t msg_len, void* d_results, void* stream) {
+    if (int e = ensure_init()) return e;
+    if (!set) return HBLS_ERR_ARG;
+    if (k == 0) return 0;
+    if (!d_index || ((uintptr_t)d_index & 3) || !d_results) return HBLS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g.mu);
+    return aggregate_verify_set_device_locked(set, k, (const uint32_t*)d_index, (const uint8_t*)d_bitmaps, (const uint8_t*)d_sigs96,
+                                              (const uint8_t*)d_msgs, msg_len, (uint8_t*)d_results, stream ? (cudaStream_t)stream : g.stream);
 }
 
 // ------------------------------------------------------------------ persistent Mask / running vote aggregate (SURVEY 8f.2)

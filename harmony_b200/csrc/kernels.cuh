@@ -111,6 +111,78 @@ __global__ void k_mask_aggregate_items(size_t B, const mask_item* __restrict__ i
     }
     if (lane == 0) out[warp] = acc;
 }
+// committee set (hbls_aggregate_verify_set_device): the mask_item descriptors built on the device from a uint32 committee index per
+// item.  Item j's bitmap starts at the sum of the bitmap bytes of items 0..j-1; an index >= m is a bad index, which occupies no
+// bitmap bytes and gets n = 0, no table and no bitmap.  The offsets are an exclusive scan across the whole batch in three launches:
+// k_set_tile_sums (one tile of HB_SET_TILE items per CTA, one item per thread), k_set_tile_scan (one CTA over the tile totals),
+// k_set_items (each tile's scan again, plus its tile's offset).
+#ifndef HB_SET_TILE
+#define HB_SET_TILE 256                     // the host emulation shrinks it so that a few dozen items span several tiles
+#endif
+enum { HB_SET_BAD_INDEX = 48 };             // == HBLS_SET_BAD_INDEX
+struct set_entry { const g1a* table; uint64_t n; };
+HB_DEV uint64_t set_item_bytes(const uint32_t* __restrict__ index, size_t j, uint32_t m, const set_entry* __restrict__ ents) {
+    const uint32_t c = index[j];
+    return c < m ? (ents[c].n + 7) >> 3 : 0;
+}
+// inclusive scan of v over the CTA (any size up to HB_SET_TILE), *total = the CTA's sum; every thread of it calls
+HB_DEV uint64_t set_cta_scan(uint64_t v, uint64_t* total) {
+    __shared__ uint64_t scan[HB_SET_TILE];
+    const unsigned t = threadIdx.x, T = blockDim.x;
+    scan[t] = v;
+    __syncthreads();
+    for (unsigned off = 1; off < T; off <<= 1) {
+        const uint64_t u = t >= off ? scan[t - off] : 0;
+        __syncthreads();
+        scan[t] += u;
+        __syncthreads();
+    }
+    const uint64_t r = scan[t];
+    *total = scan[T - 1];
+    __syncthreads();                                    // the next call may overwrite scan[]
+    return r;
+}
+// tile_sum[b] = the bitmap bytes of tile b's items
+__global__ void __launch_bounds__(HB_SET_TILE) k_set_tile_sums(size_t k, const uint32_t* __restrict__ index, uint32_t m,
+                                                              const set_entry* __restrict__ ents, uint64_t* tile_sum) {
+    const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint64_t total;
+    set_cta_scan(j < k ? set_item_bytes(index, j, m, ents) : 0, &total);
+    if (threadIdx.x == 0) tile_sum[blockIdx.x] = total;
+}
+// one CTA (any size up to HB_SET_TILE): tile_sum[0..nt) := its exclusive scan, in place
+__global__ void __launch_bounds__(HB_SET_TILE) k_set_tile_scan(size_t nt, uint64_t* tile_sum) {
+    const unsigned t = threadIdx.x, T = blockDim.x;
+    uint64_t carry = 0;
+    for (size_t b0 = 0; b0 < nt; b0 += T) {
+        const size_t b = b0 + t;
+        const uint64_t v = b < nt ? tile_sum[b] : 0;
+        uint64_t total;
+        const uint64_t incl = set_cta_scan(v, &total);
+        if (b < nt) tile_sum[b] = carry + incl - v;
+        carry += total;
+    }
+}
+// items[j] = {table, bitmaps + offset, n} of item j's committee, ok_key[j] = its index is < m
+__global__ void __launch_bounds__(HB_SET_TILE) k_set_items(size_t k, const uint32_t* __restrict__ index, uint32_t m,
+                                                          const set_entry* __restrict__ ents, const uint64_t* __restrict__ tile_off,
+                                                          const uint8_t* bitmaps, mask_item* items, uint8_t* ok_key) {
+    const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint64_t own = j < k ? set_item_bytes(index, j, m, ents) : 0;
+    uint64_t total;
+    const uint64_t incl = set_cta_scan(own, &total);
+    if (j >= k) return;
+    const uint32_t c = index[j];
+    const bool good = c < m;
+    mask_item it{nullptr, nullptr, 0};
+    if (good) { it.table = ents[c].table; it.bitmap = bitmaps + tile_off[blockIdx.x] + incl - own; it.n = ents[c].n; }
+    items[j] = it; ok_key[j] = good ? 1 : 0;
+}
+// after the verify tail: a bad index's result is HB_SET_BAD_INDEX, whatever the decode and pairing verdicts wrote
+__global__ void k_set_bad_index(size_t k, const uint8_t* __restrict__ ok_key, uint8_t* results) {
+    const size_t j = HB_TID; if (j >= k) return;
+    if (!ok_key[j]) results[j] = HB_SET_BAD_INDEX;
+}
 // large-batch form: one thread per round.  Quorum bitmaps are dense (167..250 of 250 set), so the thread sums whichever
 // side is SMALLER -- the set bits, or the unset bits subtracted from the committee total (computed once at
 // hbls_committee_create) -- from a compacted index list: ~44 point additions per round instead of ~206, and the

@@ -261,7 +261,8 @@ int hbls_verify_headers(const hbls_committee* c, size_t n, const uint8_t* sigs96
  * A graph keeps the batching regime (hbls_set_batch_mode) and the hbls_set_param values that held at capture, and the committee
  * handle must outlive every graph that uses it.  hbls_kernel_launch_count counts the launches enqueued at capture, not replays.
  * hbls_aggregate_verify_items_device cannot be captured (its descriptors come from the host array of handles): on a capturing stream
- * it returns HBLS_ERR_CAPTURE before it enqueues or allocates anything, so the capture stays valid.
+ * it returns HBLS_ERR_CAPTURE before it enqueues or allocates anything, so the capture stays valid.  Its capturable counterpart is
+ * hbls_aggregate_verify_set_device (below), whose items name their committees by an index in device memory.
  * The library's own synchronising calls (host forms, herumi-API calls, committee / mask / ballot-box calls) run in relaxed capture
  * mode, so a global-mode capture held open by another thread does not make them fail. */
 int hbls_verify_batch_status_device(size_t k, const void* d_pk48, const void* d_sig96, const void* d_msgs, size_t msg_len,
@@ -270,6 +271,30 @@ int hbls_verify_headers_device(const hbls_committee* c, size_t n, const void* d_
                                const void* d_payloads, size_t payload_len, size_t quorum, void* d_status, void* stream);
 int hbls_aggregate_verify_items_device(size_t k, const hbls_committee* const* committees, const void* d_bitmaps, const void* d_sigs96,
                                        const void* d_msgs, size_t msg_len, void* d_results, void* stream);
+
+/* Committee set: the device form of a multi-committee batch whose committees are named from device memory (crosslinks, cross-shard
+ * receipts, a multi-shard block seal: one set per (shard, epoch) table, as the reference keeps one epochCtx each).  m committee
+ * handles are registered once; their descriptors (key table, slots, bitmap bytes) are uploaded to HBM.  The committees must outlive
+ * the set, and the set must outlive every graph that uses it.  0 ok; HBLS_ERR_ARG for null out / committees, a null entry, m == 0
+ * or m > UINT32_MAX. */
+typedef struct hbls_committee_set hbls_committee_set;
+int    hbls_committee_set_create(hbls_committee_set** out, const hbls_committee* const* committees, size_t m);
+void   hbls_committee_set_destroy(hbls_committee_set* s);
+size_t hbls_committee_set_size(const hbls_committee_set* s);
+
+/* item j = (committee d_index[j] of the set, its bitmap, sig j, msg j).  d_index: k uint32, 4-byte aligned, in HBM.  Bitmaps are
+ * back to back exactly as in hbls_aggregate_verify_items: item j's bitmap starts at the sum of the bitmap bytes of items 0..j-1.
+ * d_results[j] = 1 / 0 -- byte for byte what hbls_aggregate_verify_items writes for the same items -- or HBLS_SET_BAD_INDEX when
+ * d_index[j] >= m.  Such an item occupies no bitmap bytes and does not change any other item's result.  HBLS_SET_BAD_INDEX is
+ * distinct from the HBLS_VB_*, HBLS_HDR_*, HBLS_BALLOT_* and HBLS_AGG_* codes; a caller that tests for == 1 reads it as "not valid".
+ * The per-item descriptors are built on the device (an exclusive scan of the bitmap bytes across the batch), so nothing is staged
+ * from the host: the call follows every rule of the device forms above (asynchronous on `stream`, per-stream scratch, messages
+ * grouped and hashed once each with the H(m) cache untouched, the batching regimes and hbls_last_batch_info of the items forms,
+ * stage timing), and it may be captured into a CUDA graph with no warm-up, as hbls_verify_headers_device.  0 ok (k == 0: nothing
+ * launched), HBLS_ERR_ARG for a null set, or with k > 0 a null d_index / d_results or a d_index not 4-byte aligned. */
+#define HBLS_SET_BAD_INDEX 48
+int hbls_aggregate_verify_set_device(const hbls_committee_set* set, size_t k, const void* d_index, const void* d_bitmaps,
+                                     const void* d_sigs96, const void* d_msgs, size_t msg_len, void* d_results, void* stream);
 
 /* Persistent device Mask (SURVEY 8f.2; crypto/bls/mask.go:67-242; TODO(audit) at consensus/consensus_service.go:318): the
  * bitmap lives on the host, the running aggregate public key in HBM; SetMask / SetBit apply only the DELTA (Add on 0->1,
